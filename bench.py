@@ -2,6 +2,7 @@
 """bench.py -- denoising steps/sec on 256x256 tiles of the 30m decoder U-Net (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|reference-gpu] [--tiles B] [--size S]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -39,10 +40,28 @@ METRIC = "denoising steps/sec, 256^2 latent tiles, 30m U-Net"
 UNIT = "tile-steps/s"
 SOLVE_STEPS = 20
 GFLOP_PER_STEP_256 = 343.94  # dense conv + linear FLOPs of one decoder forward at 256x256 (BASELINE.md section 2)
+DUMP_LIMIT_BYTES = 64 * 2 ** 20
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """Write each tensor as out_dir/<name>.npy in float32.  A tensor larger than its share of DUMP_LIMIT_BYTES is
+    replaced by a fixed, seeded sample of its elements; their flat indices go beside it as <name>_index.npy (float64,
+    exact below 2^53), so two builds can be compared value for value."""
+    import numpy as np
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    share = DUMP_LIMIT_BYTES // len(arrays)
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes > share:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, share // 12, replace=False))   # 4 B value + 8 B index
+            np.save(d / f"{name}_index.npy", idx.astype(np.float64))
+            a = a.reshape(-1)[idx]
+        np.save(d / f"{name}.npy", a)
 
 
 def igemm_gflop(size: int) -> float:
-    """FLOPs executed by the tcgen05 implicit-GEMM launches in one forward (everything except first/last conv, linears)."""
+    """FLOPs executed by the wgmma implicit-GEMM launches in one forward (everything except first/last conv, linears)."""
     # BASELINE.md Appendix F: 6->64 first conv 0.453, 64->1 last conv 0.075, linears 0.003 at 256^2
     return (GFLOP_PER_STEP_256 - 0.453 - 0.075 - 0.003) * (size / 256.0) ** 2
 
@@ -200,7 +219,7 @@ def run_reference_arm(args, rank):
 
 # ----------------------------------------------------------------------------------------------------- GPU reference
 def run_reference_gpu_arm(args, rank):
-    """The stated "kernel to beat" (SURVEY 8(d), BASELINE.md section 4): the reference algorithm itself on the same B200
+    """The stated "kernel to beat" (SURVEY 8(d), BASELINE.md section 4): the reference algorithm itself on the same GPU
     through PyTorch library kernels -- bf16 eager (cuDNN / cuBLAS / ATen elementwise, weight re-normalisation every
     forward, like WorldPipeline with dtype='bf16') and under torch.compile (Inductor, world_pipeline.py:421-430).  The
     reference tree cannot travel to the GPU box, so the model is its oracle restatement (bit-compatible in fp32 with the
@@ -404,7 +423,7 @@ def run_canvas_arm(args, rank, local_rank, world):
                                        f"{world} GPU(s) with neighbour strip exchange", "canvas": H, "tile": T,
                            "stride": S_, "tiles": n_tiles, "solve_steps": steps, "tile_batch": args.tile_batch,
                            "halo_bytes_per_rank_per_solve": halo, "parallelism": f"tile-row stripes x{world}",
-                           "l2": "every tile solve streams > 1 GB of activations (> 126 MB L2)"},
+                           "l2": "every tile solve streams > 1 GB of activations (> 50 MB L2)"},
                 "clocks": clk.summary(), "tflops": value * GFLOP_PER_STEP_256 * (T / 256.0) ** 2 / 1e3,
                 "owned_rows": [lo, hi]}
         print(json.dumps(line), flush=True)
@@ -504,12 +523,12 @@ def run_latent_arm(args, rank, local_rank, world):
         step_ms = ms / args.steps
         flops = GFLOP_PER_LATENT_PHASE * 1e9 * B
         achieved = flops / (step_ms * share / 1e3) / 1e12
-        peak = 1400.0
+        peak = 989.0   # H100 SXM data sheet, dense bf16 (a rated figure, not a measured one)
         try:
             peak = json.loads((ROOT / "MEASURED_PEAKS.json").read_text()).get("bf16_tflops_sustained") or peak
         except Exception:
             pass
-        roof = {"bound": "tensor", "kernel": "tdx::igemm_kernel (tcgen05 implicit-GEMM conv)", "achieved": achieved,
+        roof = {"bound": "tensor", "kernel": "tdx::igemm_kernel (wgmma implicit-GEMM conv)", "achieved": achieved,
                 "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak, "traffic": None, "launches": n_ig,
                 "kernel_share_of_step": share, "avg_launch_us": step_ms * share / n_ig * 1e3,
                 "method": "as the default arm: per-launch CUDA events give the share, x graph-replayed step time"}
@@ -640,7 +659,12 @@ def main():
                          "(configs[2]: one 1664^2 canvas, strong scaling) | export (configs[3]-shaped 9344^2 canvas)")
     ap.add_argument("--solve-steps", type=int, default=SOLVE_STEPS, help="denoising steps per tile (canvas workloads)")
     ap.add_argument("--tile-batch", type=int, default=4, help="tiles solved together per launch (canvas workloads)")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write what the last timed step returned (the denoised tiles) as "
+                         "DIR/<name>.npy, float32, at most 64 MiB (default workload only)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.workload != "tiles"):
+        ap.error("--dump-outputs is implemented for the default workload (--impl ours --workload tiles)")
     if args.warmup < 3:
         args.warmup = 3
 
@@ -720,6 +744,9 @@ def main():
         run_plan(plan, solves)         # exactly K timed steps
         e1.record()
         torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:
+        # the solver state after the last timed step = what solve.run returned to the caller
+        dump_outputs(args.dump_outputs, {"denoised": solves[plan[-1]].sample})
     if world > 1:
         dist.barrier()
     ms = e0.elapsed_time(e1)
@@ -757,7 +784,7 @@ def main():
     h2d = (noise_h.numel() + cond_h.numel()) * 4 / SOLVE_STEPS
     d2h = out_h.numel() * 4 / SOLVE_STEPS
 
-    # ---------------- roofline of the dominant kernel (tcgen05 implicit GEMM): live per-launch CUDA events
+    # ---------------- roofline of the dominant kernel (wgmma implicit GEMM): live per-launch CUDA events
     roof, cpu_base = None, None
     if rank == 0:
         s20 = get_diffusion_solve(model, sched, B, S, S, SOLVE_STEPS)
@@ -785,17 +812,13 @@ def main():
         peak = peaks.get("bf16_tflops_sustained")
         peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)"
         if not peak:
-            peak, peak_src = 1400.0, "fallback (B200_PROFILING.md sustained ~1.4 PFLOP/s)"
-        traffic = None
-        try:
-            tj = json.loads((ROOT / "profiles" / "igemm_traffic.json").read_text())
-            if tj.get("workload_tiles", 1) == args.tiles:   # the ncu capture is of the default (1-tile) workload
-                traffic = tj.get("dram_bytes_per_launch")
-        except Exception:
-            pass
-        roof = {"bound": "tensor", "kernel": "tdx::igemm_kernel (tcgen05 implicit-GEMM conv)", "achieved": achieved,
+            peak, peak_src = 989.0, "H100 SXM data sheet, dense bf16 (a rated figure, not a measured one)"
+        # bytes per launch every forward must move from DRAM at least: the bf16 weights, which exceed the 50 MB L2
+        traffic = 2 * sum(p.numel() for p in model.parameters()) * SOLVE_STEPS / n_ig
+        roof = {"bound": "tensor", "kernel": "tdx::igemm_kernel (wgmma implicit-GEMM conv)", "achieved": achieved,
                 "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak, "traffic": traffic,
                 "peak_source": peak_src, "launches": n_ig,
+                "traffic_source": "bf16 weight bytes of one forward / launches (computed, a lower bound on DRAM bytes)",
                 "avg_launch_us": ig_ms_in_graph / n_ig * 1e3,
                 "avg_launch_us_eager_events": ig_ms / n_ig * 1e3,
                 "kernel_share_of_step": share,
@@ -817,10 +840,10 @@ def main():
             "warmup": args.warmup, "ms_per_step": ms_max / args.steps, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
             "config": {"workload": f"configs[1]: 30m decoder U-Net (27.9M params), {B} x {S}x{S} tile per GPU, "
-                                   f"{SOLVE_STEPS}-step DPM-Solver++ solves, bf16 tcgen05 / fp32 accumulate",
+                                   f"{SOLVE_STEPS}-step DPM-Solver++ solves, bf16 wgmma / fp32 accumulate",
                        "tiles_per_gpu": B, "tile": S, "solve_steps": SOLVE_STEPS, "parallelism": f"tiles x{world}",
                        "l2": f"L2 flushed before the timed region; each step streams a {arena_mb:.0f} MiB activation "
-                             "arena + 56 MiB weights (> 126 MB L2), steps are data-dependent so no flush between them",
+                             "arena + 56 MiB weights (> 50 MB L2), steps are data-dependent so no flush between them",
                        "gflop_per_tile_step": GFLOP_PER_STEP_256 * (S / 256.0) ** 2},
             "clocks": clk.summary(),
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,

@@ -1,5 +1,5 @@
 /*
- * tdx.h -- C ABI of the B200-native InfiniteDiffusion sampling hot path (libtdx.so).
+ * tdx.h -- C ABI of the H100-native InfiniteDiffusion sampling hot path (libtdx.so).
  *
  * Plain C: pointers, sizes, POD structs.  No torch / C++ types cross this boundary.  Every device pointer is owned
  * by the caller unless a handle says otherwise; every launch goes to the `stream` argument (a CUstream/cudaStream_t
@@ -18,7 +18,7 @@
  *
  * Activation layout ("NC8HW8"): a [N, C, H, W] activation is stored as bf16 [N][C/8][H][W][8] -- channel groups of 8
  * (16 bytes) are the innermost unit, so a TMA box of (W-run x rows x groups) lands in shared memory exactly in the
- * tcgen05 K-major no-swizzle core-matrix order, and one thread's 8-channel store is a 16-byte vector.
+ * wgmma K-major no-swizzle core-matrix order, and one thread's 8-channel store is a 16-byte vector.
  */
 #ifndef TDX_H_
 #define TDX_H_
@@ -35,13 +35,13 @@ extern "C" {
 #define TDX_E_UNSUPPORTED -3
 
 const char* tdx_last_error(void);
-/* Library + device probe: fills sm count, compute capability; fails if the device is not sm_100. */
+/* Library + device probe: fills sm count, compute capability; fails if the device is not sm_90. */
 int tdx_device_info(int* sm_count, int* cc_major, int* cc_minor);
 /* sizeof() of the public structs (0: TdxOutSpec, 1: TdxIgemmDesc, 2: TdxConvInDesc, 3: TdxConvOutDesc, 4: TdxEmbedBlock, 5: TdxEmbedDesc, 6: TdxAttnDesc) so bindings can verify their layout. */
 int tdx_abi_sizeof(int which);
 
 /* ------------------------------------------------------------------------------------------------------------------
- * Implicit-GEMM convolution on tcgen05 (the operator under MPConv.forward, models/mp_layers.py:201-221, with the
+ * Implicit-GEMM convolution on wgmma (the operator under MPConv.forward, models/mp_layers.py:201-221, with the
  * surrounding UNetBlock elementwise math, models/unet_block.py:116-156, fused into its epilogue).
  *
  * out[m, n] = sum over segments s, taps (r,c), channels k of  A_s[pixel(m)+(r-1,c-1), k] * B[n, s, k, r, c]
@@ -100,7 +100,7 @@ int tdx_igemm_choose_n(int32_t c_out, int32_t n_img, int32_t height, int32_t wid
                        const int32_t* a_taps, int32_t n_seg);
 /* Elements of packed B for a descriptor's segments. */
 int64_t tdx_igemm_packed_weight_elems(const int32_t* a_channels, const int32_t* a_taps, int32_t n_seg, int32_t c_out);
-/* One launch of the persistent tcgen05 kernel. */
+/* One launch of the persistent wgmma kernel. */
 int tdx_igemm_run(const TdxIgemmDesc* desc, void* stream);
 
 

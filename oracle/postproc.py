@@ -9,7 +9,7 @@ What it restates (numpy float32, one function per reference function, cited by f
   * WorldPipeline._compute_climate                   terrain_diffusion/inference/world_pipeline.py:1314-1365
   * local_baseline_temperature_torch                 terrain_diffusion/inference/postprocessing.py:262-326
     (+ torch's avg_pool2d and grid_sample(bilinear, border, align_corners=False) as they are used there)
-and the two third-party pieces those call (not under /root/reference; torchvision 0.26 / torch 2.11 are installed here,
+and the two third-party pieces those call (not in the reference checkout; torchvision 0.26 / torch 2.11 are installed here,
 so the restatement is pinned against the reference run through them -- tests/golden/make_golden_post.py):
   * torchvision.transforms.functional.resize(tensor, size, BILINEAR) -> torch interpolate(mode="bilinear",
     align_corners=False, antialias=True): the separable "anti-aliased" triangle filter of ATen UpSampleKernel.cpp

@@ -11,7 +11,7 @@ Reference (xandergos/terrain-diffusion @ 82a0431):
   window-index rule of the (external) infinite_tensor canvas, black-box from call sites
                                                 world_pipeline.py:917-920,1091,1147,1230,1259-1260 (SURVEY App. C)
 
-The third-party `infinite-tensor>=0.3.0` (requirements.txt:32) is absent from /root/reference; its only arithmetic on
+The third-party `infinite-tensor>=0.3.0` (requirements.txt:32) is absent from the reference checkout; its only arithmetic on
 this path is "sum overlapping windows into an fp32 canvas, divide by the summed weight on read"
 (annotated_infinite_panorama.py:141-146), restated here as accumulate()/normalise().  PARITY UNPINNED for that
 library itself (no golden vectors exist); the bounded-canvas functions above ARE pinned against the reference by

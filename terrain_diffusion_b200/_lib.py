@@ -85,7 +85,7 @@ def lib() -> C.CDLL:
     if _lib is None:
         if not LIB_PATH.exists():
             raise TdxError(f"{LIB_PATH} not found: build it with `python -m terrain_diffusion_b200.build` "
-                           "(nvcc, sm_100a). There is no fallback path.")
+                           "(nvcc, sm_90a). There is no fallback path.")
         _lib = C.CDLL(str(LIB_PATH))
         _declare(_lib)
     return _lib

@@ -1,4 +1,4 @@
-"""Build libtdx.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libtdx.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 Usage:  python -m terrain_diffusion_b200.build [--force] [--verbose]
 The .so is written next to this file so it travels with the source tree (it is git-ignored).
@@ -17,7 +17,7 @@ LIB = PKG / "libtdx.so"
 STAMP = PKG / ".libtdx.stamp"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
     "--expt-relaxed-constexpr",
@@ -29,7 +29,7 @@ if os.environ.get("TDX_DEBUG_HOOKS") == "1":      # ablation flags / trace clock
     NVCC_FLAGS.append("-DTDX_DEBUG_HOOKS=1")
 
 
-for _flag in os.environ.get("TDX_NVCC_DEFINES", "").split():     # A/B experiments: TDX_NVCC_DEFINES="TDX_V_AHEAD_R=0 TDX_EPI_WQ=4 ..."
+for _flag in os.environ.get("TDX_NVCC_DEFINES", "").split():     # A/B experiments: TDX_NVCC_DEFINES="TDX_V_AHEAD_R=0 TDX_EPI_CHUNK=16 ..."
     NVCC_FLAGS.append("-D" + _flag)
 
 

@@ -24,7 +24,7 @@ int sm_count() {
   if (dev < 0 || dev >= 16) dev = 0;
   if (n[dev] == 0) {
     cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (n[dev] <= 0) n[dev] = 148;
+    if (n[dev] <= 0) n[dev] = 132;
   }
   return n[dev];
 }
@@ -116,8 +116,8 @@ extern "C" int tdx_device_info(int* sm_count_out, int* cc_major, int* cc_minor) 
   if (sm_count_out) *sm_count_out = sms;
   if (cc_major) *cc_major = major;
   if (cc_minor) *cc_minor = minor;
-  if (major != 10) {
-    tdx::set_error("libtdx is built for sm_100a only; device reports compute capability %d.%d", major, minor);
+  if (major != 9 || minor != 0) {
+    tdx::set_error("libtdx is built for sm_90a only; device reports compute capability %d.%d", major, minor);
     return TDX_E_UNSUPPORTED;
   }
   return TDX_OK;

@@ -1,31 +1,28 @@
-// Persistent, warp-specialised implicit-GEMM convolution for sm_100a.
+// Persistent, warp-specialised implicit-GEMM convolution for sm_90a.
 //
-//   D[128 pixels x 64 channels] (fp32, TMEM) += A[128 x 16] (bf16, smem halo patch) * B[64 x 16] (bf16, smem weights)
+//   D[128 pixels x N channels] (fp32) += A[128 x 16] (bf16, smem halo patch) * B[N x 16] (bf16, smem weights)
 //
-// * Work item = (M tile of 16 rows x 8 columns of output pixels) x (64-channel slice of Cout).  The slices of one
-//   M tile are adjacent work items, so they run concurrently on neighbouring CTAs and share the A patch in L2; small
-//   layers (32x32, 64x64 resolution) get Cout/64 times more CTAs this way.
+// * Work item = (M tile of 16 rows x 8 columns of output pixels) x (N-channel slice of Cout, N = 64 .. 256).  The
+//   slices of one M tile are adjacent work items, so they run concurrently on neighbouring CTAs and share the A patch
+//   in L2; small layers (32x32, 64x64 resolution) get Cout/N times more CTAs this way.
 // * The A operand of every filter tap is the SAME (18 x 10)-pixel halo patch in shared memory: activations are stored
-//   NC8HW8, so TMA drops the patch as [kc][18][10][8ch] and the tcgen05 K-major/no-swizzle descriptor (8-row core
+//   NC8HW8, so TMA drops the patch as [kc][18][10][8ch] and the wgmma K-major/no-swizzle descriptor (8-row core
 //   matrices 128 B contiguous, SBO = 10 px * 16 B between pixel rows, LBO = one 8-channel plane) addresses tap (r,c)
 //   by just adding (r*10+c)*16 B to the start address.  The patch is fetched once per 64-channel chunk and used by all
 //   9 taps (1.4x halo overhead instead of 9x re-fetch); conv zero padding is TMA out-of-bounds fill.
-// * B (weights) are pre-packed on the host in exactly the shared-memory image order, one 8 KB stage per (chunk, tap),
-//   and streamed with 1-D bulk copies through their own ring.
-// * A K=16 tcgen05.mma has ~105 cycles of issue-to-issue latency when it accumulates into the tile the previous MMA
-//   wrote (measured: N=64 MMAs ran at 106 cycles instead of their 32-cycle throughput floor).  The four K=16 steps
-//   of a stage therefore accumulate into FOUR independent TMEM accumulators (4 x 64 columns) that the epilogue sums,
-//   so consecutive MMAs never depend on each other.  2 x (4 x 64) columns = all 512 TMEM columns, double-buffered so
-//   the epilogue of item i overlaps the MMAs of item i+1.
-// * Warp roles (all warp-converged, single-issuer instructions predicated on one elected lane): w0 A-producer (TMA
-//   tiled), w1 B-producer (bulk copy), w2 MMA issuer, w3 TMEM allocator, w4..w11 epilogue (two warps per TMEM lane
-//   quadrant, one 32-column chunk each).
+// * B (weights) are pre-packed on the host in exactly the shared-memory image order, one stage per (chunk, tap), and
+//   streamed with 1-D bulk copies through their own ring.
+// * Warp roles: w0 A-producer (TMA tiled), w1 B-producer (bulk copy), w2 barrier set-up, w4..w11 two consumer
+//   warpgroups.  Warpgroup g issues m64nNk16 wgmmas for pixels 64g .. 64g+63 (tile rows 8g .. 8g+7) with the
+//   accumulator in registers, then writes it to a shared-memory staging tile (fp32, [channel][pixel]) from which all
+//   eight warps run the epilogue with one thread per pixel.  The producers keep filling the rings for the next item
+//   while the epilogue runs.
 // * Epilogue: each thread owns one pixel; it applies emb-scale+mp_silu / residual mp_sum + clip / pixel-norm and
 //   writes up to three bf16 NC8HW8 outputs (raw, activated, activated+resampled) for the consumers.  Pixel-norm needs
-//   the sum of squares over ALL Cout channels: the Cout/64 CTAs of one M tile are then launched as a thread-block
+//   the sum of squares over ALL Cout channels: the Cout/N CTAs of one M tile are then launched as a thread-block
 //   cluster and exchange their per-pixel partial sums through distributed shared memory + a cluster-scope mbarrier.
-// * Programmatic dependent launch: barrier init, TMEM allocation, descriptor prefetch and the weight stream of kernel
-//   N+1 overlap the tail of kernel N; griddepcontrol.wait guards everything that depends on earlier kernels.
+// * Programmatic dependent launch: barrier init, descriptor prefetch and the weight stream of kernel N+1 overlap the
+//   tail of kernel N; griddepcontrol.wait guards everything that depends on earlier kernels.
 //
 // Reference math being replaced: models/mp_layers.py:201-221 (MPConv), models/unet_block.py:116-156 (UNetBlock).
 #include <stdlib.h>
@@ -39,23 +36,22 @@ constexpr int kTileH = 16, kTileW = 8;
 constexpr int kPatchH = kTileH + 2, kPatchW = kTileW + 2;
 constexpr int kKcBytes = kPatchH * kPatchW * 16;  // one 8-channel plane of the halo patch: 2880 B
 constexpr int kAStageBytes = 8 * kKcBytes;        // 64 channels: 23040 B
-constexpr int kSA = 3;                            // A ring depth
+constexpr int kSA = 3;                            // A ring depth (max; 2 when the staging tile leaves no room)
 constexpr int kMaxSB = 18;                        // B ring depth (max; also the largest resident weight set)
-constexpr int kAccCols = 256;                     // TMEM columns per accumulator buffer (2 buffers)
-#ifndef TDX_EPI_WQ
-#define TDX_EPI_WQ 2
-#endif
 #ifndef TDX_EPI_CHUNK
 #define TDX_EPI_CHUNK 32
 #endif
-constexpr int kWQ = TDX_EPI_WQ;                   // epilogue warps per TMEM lane quadrant (2 or 4)
-constexpr int kEpiWarps = 4 * kWQ;
+constexpr int kWQ = 2;                            // epilogue warps per 32-pixel quadrant
+constexpr int kEpiWarps = 4 * kWQ;                // = the two consumer warpgroups
 constexpr int kChunk = TDX_EPI_CHUNK;             // accumulator columns an epilogue warp handles at a time (16 or 32)
 constexpr int kGroups = kChunk / 8;               // 8-channel groups (one uint4 of bf16) per chunk
 constexpr int kThreads = 128 + 32 * kEpiWarps;
 constexpr int kMaxSplit = 8;                      // max CTAs (cluster size) sharing one M tile's pixel-norm statistics
-constexpr int kSmemMisc = 14336;                  // barriers, TMEM slot, pixel-norm statistics
+constexpr int kSmemMisc = 14336;                  // barriers, pixel-norm statistics
 constexpr int kSmemBudget = 227 * 1024;
+// Staging tile row pitch in floats: the 4 lanes of a wgmma fragment quad write channels 2 apart, 264 words = 8 banks
+// apart, so a warp's fragment store and the epilogue's per-pixel loads are both free of bank conflicts.
+constexpr int kStgLd = 132;
 
 // Division by a launch constant with a host-made reciprocal: exact while n * d < 2^32 (all uses divide blockIdx.x-sized
 // numbers); keeps runtime integer divisions (~150 cycles each) off the launch's critical path.
@@ -78,6 +74,7 @@ struct IgemmParams {
   int cout, nsplit;
   float inv_cout;
   int ncta;                   // output channels per work item = MMA N (64, 128, 192 or 256); cout = ncta * nsplit
+  int SA;                     // A ring depth
   int SB;                     // B ring depth
   int b_stage_bytes;          // ncta * 128
   int resident;               // the whole weight set of an item fits the ring: loaded once per CTA, reused by every item
@@ -123,7 +120,7 @@ __device__ __forceinline__ void stage_locate(const IgemmParams& p, int s, int& s
 #ifndef TDX_DEBUG_HOOKS
 #define TDX_DEBUG_HOOKS 0
 #endif
-// A/B switches of measured experiments (profiles/r02_epilogue_stalls.txt; set through TDX_NVCC_DEFINES, see build.py):
+// A/B switches (set through TDX_NVCC_DEFINES, see build.py):
 //   TDX_V_TWO_KERNELS  launches without clusters use the cluster-free instantiation (0: one kernel for everything)
 //   TDX_V_AHEAD_R / _C residual / modulation vector fetched one item ahead (R: 0 = at the item's start; C: 0 = in place,
 //                      1 = at the item's start, 2 = one item ahead)
@@ -219,20 +216,11 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-// ---------------------------------------------------------------------------------------------- issue helpers
-// A value every lane already agrees on, moved into a UNIFORM register (REDUX writes its result there), so that
-// arithmetic on it stays on the uniform datapath and instructions with uniform operands (UTCHMMA) need no R2UR.
-__device__ __forceinline__ uint32_t uni(uint32_t v) { return __reduce_or_sync(0xffffffffu, v); }
-__device__ __forceinline__ uint64_t pack_desc(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
-
 // ---------------------------------------------------------------------------------------------- epilogue helpers
-__device__ __forceinline__ void load_acc(uint32_t taddr, float (&v)[kChunk]) {
-  uint32_t r[kChunk];
-  if constexpr (kChunk == 32) tmem_ld32(taddr, reinterpret_cast<uint32_t(&)[32]>(r));
-  else tmem_ld16(taddr, reinterpret_cast<uint32_t(&)[16]>(r));
-  tmem_ld_wait();
+// kChunk accumulator columns from `col` of pixel m, out of the staging tile
+__device__ __forceinline__ void load_acc(const float* stg, int m, int col, float (&v)[kChunk]) {
 #pragma unroll
-  for (int i = 0; i < kChunk; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < kChunk; ++i) v[i] = stg[(col + i) * kStgLd + m];
 }
 
 // 1 / (eps + sqrt(mean square)) with the two MUFU approximations (relative error ~2^-22: invisible after bf16 rounding)
@@ -283,9 +271,98 @@ __device__ __forceinline__ void store_chunk(uint4* dst, uint32_t plane, int Wo, 
   }
 }
 
+// Ring positions of the consumer warpgroups (every consumer thread keeps the same copy).
+struct ConsumerRing {
+  int sa, sb;
+  uint32_t pha;     // a_full parity
+  uint32_t fmask;   // expected parity of every b_full barrier (a hand-over group's barrier = its first slot's)
+};
+
+// One work item's K stages [s0, s1) on the tensor cores.  Consumer warpgroup wg computes pixels 64 wg .. 64 wg + 63
+// against all kN channels of the item, then stores its accumulator into the staging tile stg[channel * kStgLd + pixel].
+template <int kN>
+__device__ __forceinline__ void mma_item(const IgemmParams& p, const uint8_t* a_ring, const uint8_t* b_ring,
+                                         uint64_t* a_full, uint64_t* a_empty, uint64_t* b_full, uint64_t* b_empty,
+                                         ConsumerRing& r, int s0, int s1, bool steady, float* stg) {
+  const int lane = threadIdx.x & 31, wl = (threadIdx.x >> 5) & 3, wg = (int)(threadIdx.x >> 7) - 1;
+  float acc[kN / 2];
+#pragma unroll
+  for (int i = 0; i < kN / 2; ++i) acc[i] = 0.f;
+  constexpr uint32_t b_lbo = kN * 16;
+  const uint32_t a_base = smem_u32(a_ring) + wg * 8 * kPatchW * 16;
+  const uint32_t b_base = smem_u32(b_ring);
+  // A stage's ring slots are released one stage late, so one stage is in flight while the next is issued.  A one-slot
+  // weight ring cannot wait like that: its only slot is the one the next stage needs.
+  const bool deep = p.SB > 1 || p.resident;
+  int pend_a = -1, pend_b = -1;
+  auto release = [&](int a, int b) {
+    __syncwarp();
+    if (lane == 0) {
+      if (b >= 0) mbar_arrive(&b_empty[b]);
+      if (a >= 0) mbar_arrive(&a_empty[a]);
+    }
+  };
+  for (int s = s0; s < s1;) {
+    int seg, ch, tap0, taps;
+    stage_locate(p, s, seg, ch, tap0, taps);
+    const int tap1 = (taps - tap0 < s1 - s) ? taps : tap0 + (s1 - s);
+    const int nt = tap1 - tap0;
+    s += nt;
+    mbar_wait(&a_full[r.sa], r.pha);
+    const uint32_t a_stage = a_base + r.sa * kAStageBytes;
+    // tap offsets (r * 10 + c pixels) come from a packed table, 5 bits per tap; a 1x1 segment reads the patch centre
+    unsigned long long tt = taps == 9 ? (0x16ad18b50820ull >> (5 * tap0)) : (unsigned long long)(kPatchW + 1);
+    // hand-over groups of up to `bgroup` taps (one group = everything when the weights are already resident)
+    const int gsz = steady ? nt : p.bgroup;
+    int t = 0;
+    for (int g0 = 0; g0 < nt; g0 += gsz) {
+      const int gn = nt - g0 < gsz ? nt - g0 : gsz;
+      if (!steady) {
+        mbar_wait(&b_full[r.sb], (r.fmask >> r.sb) & 1u);
+        r.fmask ^= 1u << r.sb;
+      }
+      for (int k = 0; k < gn; ++k, ++t, tt >>= 5) {
+        const uint32_t al = a_stage + (uint32_t)(tt & 31ull) * 16;
+        const uint32_t bl = b_base + r.sb * p.b_stage_bytes;
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          wgmma_bf16<kN>(acc, make_smem_desc(al + j * 2 * kKcBytes, kKcBytes, kPatchW * 16),
+                         make_smem_desc(bl + j * 2 * b_lbo, b_lbo, 128), 1u);
+        wgmma_commit();
+        const int rel_b = p.resident ? -1 : r.sb;
+        const int rel_a = t == nt - 1 ? r.sa : -1;   // the chunk's last tap frees its halo patch
+        if (deep) {
+          wgmma_wait<1>();
+          release(pend_a, pend_b);
+          pend_a = rel_a;
+          pend_b = rel_b;
+        } else {
+          wgmma_wait<0>();
+          release(rel_a, rel_b);
+        }
+        if (++r.sb == p.SB) r.sb = 0;
+      }
+    }
+    if (++r.sa == p.SA) { r.sa = 0; r.pha ^= 1; }
+  }
+  wgmma_wait<0>();
+  release(pend_a, pend_b);
+  named_bar_sync(13, 32 * kEpiWarps);   // the previous item's epilogue has read the staging tile
+  float* dst = stg + 64 * wg + 16 * wl + (lane >> 2);
+#pragma unroll
+  for (int j = 0; j < kN / 8; ++j)
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int c = 0; c < 2; ++c) dst[(8 * j + 2 * (lane & 3) + c) * kStgLd + 8 * i] = acc[4 * j + 2 * i + c];
+  named_bar_sync(13, 32 * kEpiWarps);
+}
+
 // kCL = the launch uses clusters (split-K and / or pixel-norm statistics across CTAs).  The many-item launches do not:
 // their instantiation carries none of that code (a shorter epilogue loop, fewer instruction-cache misses).
-template <bool kCL>
+// kN = output channels per work item (the wgmma N).
+template <bool kCL, int kN>
 __global__ void __launch_bounds__(kThreads, 1)
 igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
              const __grid_constant__ CUtensorMap tm2, const __grid_constant__ IgemmParams p) {
@@ -293,24 +370,21 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
   const int ksplit_ = kCL ? p.ksplit : 1;
   const bool cstats_ = kCL && p.cluster_stats;
   uint8_t* a_ring = smem;
-  uint8_t* b_ring = smem + kSA * kAStageBytes;
+  uint8_t* b_ring = smem + p.SA * kAStageBytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(b_ring + p.SB * p.b_stage_bytes);
   uint64_t* a_full = bars;
   uint64_t* a_empty = a_full + kSA;
   uint64_t* b_full = a_empty + kSA;
   uint64_t* b_empty = b_full + kMaxSB;
-  uint64_t* t_full = b_empty + kMaxSB;
-  uint64_t* t_empty = t_full + 2;
-  uint64_t* x_full = t_empty + 2;                                     // [2] cluster statistics barriers
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(x_full + 2);
+  uint64_t* x_full = b_empty + kMaxSB;                                // [2] cluster statistics barriers
   float* ssq = reinterpret_cast<float*>(bars) + 256;                  // [4 epilogue warps of a pixel][128 pixels]
   float* rss = ssq + 512;                                             // same, for the residual's pixel-norm
   float* stot = rss + 512;                                            // [128] per-pixel totals over the cluster
   float* xstat = stot + 128;                                          // [2 parity][kMaxSplit][128] from peer CTAs
+  float* stg = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + kSmemMisc);   // [kN][kStgLd] accumulator
 
   // The role id goes through a shuffle so that ptxas KNOWS it is warp-uniform: with a plain threadIdx.x >> 5 the role
-  // branches count as divergent regions (code follows them), and inside a divergent region nothing is kept in uniform
-  // registers -- every UTCHMMA / TMA / mbarrier operand then costs an R2UR.
+  // branches count as divergent regions, and inside a divergent region nothing is kept in uniform registers.
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const int lane = threadIdx.x & 31;
 #if TDX_DEBUG_HOOKS
@@ -328,32 +402,25 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
     if (p.nseg > 2) tma_prefetch_desc(&tm2);
   }
   if (warp == 2) {
-    // all 48 barriers at once, two per lane (one thread initialising them in turn costs ~800 cycles of every launch):
-    // [a_full 3][a_empty 3][b_full 18][b_empty 18][t_full 2][t_empty 2][x_full 2], contiguous from `bars`
-    constexpr int kBars = 2 * kSA + 2 * kMaxSB + 6;
+    // all 44 barriers at once, two per lane (one thread initialising them in turn costs ~800 cycles of every launch):
+    // [a_full 3][a_empty 3][b_full 18][b_empty 18][x_full 2], contiguous from `bars`.  Every consumer warp frees a slot.
+    constexpr int kBars = 2 * kSA + 2 * kMaxSB + 2;
     static_assert(kBars <= 64, "two barriers per lane");
-    const int t_empty0 = 2 * kSA + 2 * kMaxSB + 2;
+    const int x_full0 = 2 * kSA + 2 * kMaxSB;
 #pragma unroll
     for (int k = 0; k < 2; ++k) {
       const int i = lane + 32 * k;
       if (i < kBars) {
         uint32_t count = 1;
-        if (i >= t_empty0 && i < t_empty0 + 2) count = kEpiWarps;
-        if (i >= t_empty0 + 2) count = p.xsplit > 1 ? (uint32_t)(p.xsplit - 1) * 128u : 1u;
+        if ((i >= kSA && i < 2 * kSA) || (i >= 2 * kSA + kMaxSB && i < x_full0)) count = kEpiWarps;
+        if (i >= x_full0) count = p.xsplit > 1 ? (uint32_t)(p.xsplit - 1) * 128u : 1u;
         mbar_init(&bars[i], count);
       }
     }
     fence_mbar_init();
   }
-  if (warp == 3) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   if (cstats_) cluster_sync_all();   // peers' barriers are initialised before anyone arrives on them
-  const uint32_t tmem_base = *tmem_slot;
 #if TDX_DEBUG_HOOKS
   if (p.trace && blockIdx.x == 0 && threadIdx.x == 0) p.trace[127] = clock64();
 #endif
@@ -377,13 +444,13 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
         int seg, ch, tap, taps;
         stage_locate(p, s, seg, ch, tap, taps);
         const CUtensorMap* tm = seg == 0 ? &tm0 : (seg == 1 ? &tm1 : &tm2);
-        mbar_wait(&a_empty[sa], ph ^ 1, 100 + sa);
+        mbar_wait(&a_empty[sa], ph ^ 1);
         if (elect_one()) {
           mbar_expect_tx(&a_full[sa], kAStageBytes);
           tma_load_4d(tm, &a_full[sa], a_ring + sa * kAStageBytes, (X0 - 1) * 8, Y0 - 1, ch * 8, img);
         }
         __syncwarp();
-        if (++sa == kSA) { sa = 0; ph ^= 1; }
+        if (++sa == p.SA) { sa = 0; ph ^= 1; }
         s += taps - tap;   // the rest of this chunk's taps use the same patch
       }
     }
@@ -409,7 +476,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
         // stage-by-stage hand-over (streaming rings): the tightest loop possible -- at N >= 128 this warp has to issue a
         // stage every ~256 cycles, and an mbarrier try_wait alone costs ~90
         for (int ks = 0; ks < st1 - st0; ++ks) {
-          mbar_wait(&b_empty[sb], ph ^ 1, 200 + sb);
+          mbar_wait(&b_empty[sb], ph ^ 1);
           if (elect_one()) {
             if (TDX_DBG(2)) {
               mbar_arrive(&b_full[sb]);
@@ -431,7 +498,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
         const int nt = (taps - tap0 < st1 - s) ? taps - tap0 : st1 - s;
         int head = sb, gi = 0;
         for (int t = 0; t < nt; ++t) {
-          if (!p.resident) mbar_wait(&b_empty[sb], ph ^ 1, 200 + sb);
+          if (!p.resident) mbar_wait(&b_empty[sb], ph ^ 1);
           const bool first = gi == 0;                        // first stage of a hand-over group: its barrier carries the group
           if (++gi == p.bgroup) gi = 0;                      // (no integer division in this loop: ~150 cycles each)
           if (first) head = sb;
@@ -454,111 +521,12 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
       if (p.resident) break;   // the ring now holds this CTA's whole weight slice for every later item
     }
     if (ksplit_ > 1) cluster_sync_all();
-  } else if (warp == 2) {
-    // ------------------------------------------------------------------ MMA issuer (one elected lane issues)
-    // Everything a UTCHMMA reads (two 64-bit matrix descriptors, the TMEM address, the instruction descriptor) lives
-    // in UNIFORM registers.  ptxas only keeps a value there when it can prove it warp-uniform, and a value that
-    // passed through a per-thread register (shared-memory loads, the ring counters of a loop with a spin-wait in it)
-    // costs an R2UR per use: the round-1 loop spent ~70-86 cycles of issue per MMA on R2UR / uniform-register spills,
-    // while the tensor pipe needs 48 (N=64), 64 (N=128), 96 (N=192), 128 (N=256) cycles (tools/probe/mma_probe3.cu).
-    // So every loop-carried quantity below is seeded from a warp reduction (REDUX writes a uniform register) and only
-    // updated with uniform arithmetic; descriptors are (constant upper word, low word = base + compile-time offset).
-    const uint32_t idesc = uni(make_idesc_bf16(128, p.ncta));
-    const uint32_t b_lbo = p.ncta * 16;
-    const uint32_t a_sbo = TDX_DBG(1) ? 128 : kPatchW * 16;
-    const uint64_t a_hi = make_smem_desc(0, kKcBytes, a_sbo);
-    const uint64_t b_hi = make_smem_desc(0, b_lbo, 128);
-    const uint32_t a_h = uni((uint32_t)(a_hi >> 32)), b_h = uni((uint32_t)(b_hi >> 32));
-    // (in a cluster launch the shared-window address carries the CTA rank in its upper bits: keep the 14-bit field only)
-    const uint32_t a_lo0 = uni((uint32_t)a_hi + ((smem_u32(a_ring) >> 4) & 0x3FFF));
-    const uint32_t b_lo0 = uni((uint32_t)b_hi + ((smem_u32(b_ring) >> 4) & 0x3FFF));
-    const uint32_t b_stage16 = uni((uint32_t)p.b_stage_bytes >> 4), b_kstep16 = uni((2 * b_lbo) >> 4);
-    constexpr uint32_t a_kstep16 = (2 * kKcBytes) >> 4;
-    const uint32_t tmem_u = uni(tmem_base);
-    const uint32_t SBu = uni((uint32_t)p.SB);
-    const uint32_t resident = uni((uint32_t)p.resident);
-    const uint32_t bgroup = uni((uint32_t)p.bgroup);
-    uint32_t sa = uni(0), sb = uni(0);
-    uint32_t pha = 0;
-    uint32_t fmask = uni(0);   // expected parity of every b_full barrier (a group's barrier = its first slot's)
-    uint32_t it = uni(0);
-    int s0, s1;
-    {
-      const uint32_t bk = fdiv(blockIdx.x, p.fd_ks);
-      stage_range(p, (int)(blockIdx.x - bk * p.fd_ks.d), s0, s1);
-      s0 = (int)uni((uint32_t)s0);
-      s1 = (int)uni((uint32_t)s1);
-    }
-    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x, ++it) {
-      const uint32_t acc = it & 1;
-      const uint32_t accph = (it >> 1) & 1;
-      mbar_wait(&t_empty[acc], accph ^ 1, 300 + acc);
-      tc_fence_after();
-      if (lane == 0) TDX_TRACE(1, it);
-      const uint32_t d_tmem = uni(tmem_u + acc * kAccCols);
-      const bool steady = resident && it > 0;   // weights already in the ring: no per-stage handshakes
-      uint32_t accumulate = uni(0);
-      for (int s = s0; s < s1;) {
-        int seg, ch, tap0, taps;
-        stage_locate(p, s, seg, ch, tap0, taps);
-        // (the segment table is indexed dynamically, which ptxas cannot prove uniform: re-seed what the loop carries)
-        tap0 = (int)uni((uint32_t)tap0);
-        taps = (int)uni((uint32_t)taps);
-        const int tap1 = (taps - tap0 < s1 - s) ? taps : tap0 + (s1 - s);
-        mbar_wait(&a_full[sa], pha, 400 + sa);
-        tc_fence_after();
-        if (lane == 0 && s == s0) TDX_TRACE(2, it);
-        s += tap1 - tap0;
-        const uint32_t a_lo = a_lo0 + sa * (kAStageBytes >> 4);
-        const uint32_t nt = (uint32_t)(tap1 - tap0);
-        // tap offsets (r * 10 + c pixels) come from a packed table, 5 bits per tap; a 1x1 segment reads the patch centre
-        const unsigned long long taptab = taps == 9 ? (0x16ad18b50820ull >> (5 * tap0)) : (unsigned long long)(kPatchW + 1);
-        // ---- hand-over groups of up to `bgroup` taps (one group = everything when the weights are already resident)
-        const uint32_t gsz = steady ? nt : bgroup;
-        unsigned long long tt = taptab;
-        for (uint32_t g0 = 0; g0 < nt; g0 += gsz) {
-          const uint32_t gn = nt - g0 < gsz ? nt - g0 : gsz;
-          if (!steady) {
-            mbar_wait(&b_full[sb], (fmask >> sb) & 1u, 500 + sb);
-            tc_fence_after();
-            fmask ^= 1u << sb;
-          }
-          if (elect_one()) {
-            uint32_t slot = sb, bl = b_lo0 + sb * b_stage16;
-            unsigned long long t2 = tt;
-#pragma unroll 1
-            for (uint32_t t = 0; t < gn; ++t, t2 >>= 5) {
-              const uint32_t al = a_lo + (uint32_t)(t2 & 31ull);
-#pragma unroll
-              for (int j = 0; j < 4; ++j)
-                umma_bf16(d_tmem, pack_desc(al + j * a_kstep16, a_h), pack_desc(bl + j * b_kstep16, b_h), idesc,
-                          (accumulate | t | j) ? 1u : 0u);
-              if (!resident) umma_commit(&b_empty[slot]);
-              bl += b_stage16;
-              if (++slot == SBu) { slot = 0; bl = b_lo0; }
-            }
-          }
-          __syncwarp();
-          accumulate = 1;
-          tt >>= 5 * gn;
-          sb += gn;
-          if (sb >= SBu) sb -= SBu;
-        }
-        if (elect_one()) umma_commit(&a_empty[sa]);
-        __syncwarp();
-        if (++sa == kSA) { sa = 0; pha ^= 1; }
-      }
-      if (elect_one()) umma_commit(&t_full[acc]);
-      __syncwarp();
-      if (lane == 0) TDX_TRACE(3, it);
-    }
+  } else if (warp < 4) {
     if (ksplit_ > 1) cluster_sync_all();
-  } else if (warp == 3) {
-    if (ksplit_ > 1) cluster_sync_all();
-  } else if (warp >= 4 && !TDX_DBG(8)) {
-    // ------------------------------------------------------------------ epilogue (TMEM -> registers -> global)
-    // Warp w reads TMEM lane quadrant q = w & 3 (pixels q*32 .. q*32+31, one per lane); the kWQ warps of a quadrant
-    // (wq = 0 .. kWQ-1) take the item's kChunk-column chunks round-robin.
+  } else {
+    // ------------------------------------------------------------------ consumers: MMA, then the epilogue
+    // In the epilogue warp w handles quadrant q = w & 3 of the staging tile (pixels q*32 .. q*32+31, one per lane); the
+    // kWQ warps of a quadrant (wq = 0 .. kWQ-1) take the item's kChunk-column chunks round-robin.
     pdl_wait();  // residual / cvec come from earlier kernels; our stores must not race their readers
     const int q = warp & 3;
     const int wq = (warp - 4) >> 2;
@@ -571,6 +539,9 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
     const uint32_t my_rank = cstats_ ? cluster_ctarank() : 0;
     TileWalk tw;
     tw.init(p);
+    ConsumerRing ring = {0, 0, 0u, 0u};
+    int s0, s1;
+    stage_range(p, tw.kpart, s0, s1);
     // Per-CTA constants: with split-K (one item per CTA) this part finalises `slice` of the item's columns.
     const int ks = ksplit_, kpart = tw.kpart;
     const int slice = p.ncta / ks, sch = slice / kChunk;
@@ -630,9 +601,8 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
     }
     // The values an item needs from global memory before it can touch its accumulator are requested ONE ITEM AHEAD
     // (`fetch_ahead`, called where the current item has consumed them): the residual's first-chunk channels or the
-    // modulation vector's first chunk (`pre`) and the residual's pixel-norm factor (`rinv_pre`).  Requested at the start of
-    // their own item, the factor alone cost 25-29 % of the epilogue of the residual layers (long-scoreboard stall on
-    // its first use, ncu source view, profiles/r02_epilogue_stalls.txt).
+    // modulation vector's first chunk (`pre`) and the residual's pixel-norm factor (`rinv_pre`), so that their first use
+    // does not wait on a global load.
     constexpr int kPreN = (kChunk / 4 > kGroups) ? kChunk / 4 : kGroups;
     uint4 pre[kPreN];
     const uint4* rbase_pre = nullptr;
@@ -661,12 +631,12 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
     if (ahead) fetch_ahead(tw);
     int it = 0;
     for (int item = blockIdx.x; item < p.num_items; item += gridDim.x, ++it, tw.next(p)) {
-      const int acc = it & 1;
-      const uint32_t accph = (it >> 1) & 1;
       const int img = tw.img;
       const int Y = tw.ty * kTileH + y, X = tw.tx * kTileW + x;
       const bool valid = (Y < p.H) && (X < p.W);
-      const uint32_t taddr = tmem_base + acc * kAccCols + ((uint32_t)(q * 32) << 16);
+      if (warp == 4 && lane == 0) TDX_TRACE(1, it);
+      mma_item<kN>(p, a_ring, b_ring, a_full, a_empty, b_full, b_empty, ring, s0, s1, p.resident && it > 0, stg);
+      if (warp == 4 && lane == 0) TDX_TRACE(2, it);
 
       // ---------------- split-K: the ksplit CTAs of a cluster each hold a partial sum of the same 128 x ncta tile.
       // Reduce-scatter through an L2-resident fp32 workspace: every part publishes the column slices the other parts
@@ -675,9 +645,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
       const float* red_src = nullptr;
       if (ks > 1) {
         float* wsg = p.ws + (size_t)fdiv((uint32_t)item, p.fd_ks) * (ks - 1) * p.ncta * 128;   // [dst part][source slot][slice cols][128]
-        mbar_wait(&t_full[acc], accph, 600 + acc);
-        tc_fence_after();
-        if (warp == 4 && lane == 0) TDX_TRACE(7, it);
+        if (warp == 4 && lane == 0) TDX_TRACE(3, it);
         for (int ck = wq; ck < nchunks_all; ck += kWQ) {
           const int dst = ck / sch;
           if (dst == kpart) continue;
@@ -685,14 +653,13 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
           float* d = wsg + ((size_t)(dst * (ks - 1) + slot) * slice + (size_t)(ck - dst * sch) * kChunk) * 128 + m;
           float v[kChunk];
           __syncwarp();
-          load_acc(taddr + ck * kChunk, v);
+          load_acc(stg, m, ck * kChunk, v);
 #pragma unroll
           for (int j = 0; j < kChunk; ++j) __stcg(d + (size_t)j * 128, v[j]);
         }
         cluster_sync_all();
         red_src = wsg + (size_t)kpart * (ks - 1) * slice * 128 + m;
       }
-      const uint32_t taddr_e = taddr + col0;
       const float* cvb = p.cvec ? p.cvec + (size_t)img * p.cout + chbase : nullptr;
       // adds the other parts' partial sums to this CTA's chunk ck (no-op without split-K)
       auto add_partials = [&](int ck, float (&v)[kChunk]) {
@@ -747,15 +714,11 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
           optr[o] = reinterpret_cast<uint4*>(p.out[o].ptr) + item_off(ospec[o], tw);
         }
 
-        if (warp == 4 && lane == 0) TDX_TRACE(4, it);
-        mbar_wait(&t_full[acc], accph, 600 + acc);
-        tc_fence_after();
-        if (warp == 4 && lane == 0) TDX_TRACE(5, it);
 
         // v = accumulator chunk `ck` after emb-silu / residual / clip (everything that precedes the pixel-norm)
         auto compute_v = [&](int ck, float (&v)[kChunk]) {
           __syncwarp();
-          load_acc(taddr_e + ck * kChunk, v);
+          load_acc(stg, m, col0 + ck * kChunk, v);
           add_partials(ck, v);
           if (p.epi & TDX_EPI_EMB_SILU) {
 #pragma unroll
@@ -825,7 +788,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
               if (!mbar_try_wait_cluster(&x_full[par], xph)) {
                 const long long t0 = clock64();
                 while (!mbar_try_wait_cluster(&x_full[par], xph)) {
-                  if (clock64() - t0 > TDX_WAIT_LIMIT) mbar_timeout(700 + par, xph);
+                  if (clock64() - t0 > TDX_WAIT_LIMIT) asm volatile("trap;");
                 }
               }
               for (uint32_t r = 0; r < (uint32_t)p.xsplit; ++r)
@@ -869,20 +832,12 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&t_empty[acc]);
-      if (warp == 4 && lane == 0) TDX_TRACE(6, it);
+      if (warp == 4 && lane == 0) TDX_TRACE(4, it);
     }
   }
 
-  tc_fence_before();
   __syncthreads();
   if (cstats_) cluster_sync_all();   // nobody leaves while a peer may still write into its shared memory
-  if (warp == 3) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 #if TDX_DEBUG_HOOKS
   if (p.trace && blockIdx.x == 0 && threadIdx.x == 96) p.trace[125] = clock64();
   if (p.timeline && threadIdx.x == 0) {
@@ -901,11 +856,24 @@ static int g_dbg_flags = 0;
 
 static int ensure_scratch(float** ws);
 
+typedef decltype(&igemm_kernel<false, 64>) IgemmKernel;
+
+static IgemmKernel igemm_kernel_for(bool cluster, int n) {
+  switch (n) {
+    case 64: return cluster ? igemm_kernel<true, 64> : igemm_kernel<false, 64>;
+    case 128: return cluster ? igemm_kernel<true, 128> : igemm_kernel<false, 128>;
+    case 192: return cluster ? igemm_kernel<true, 192> : igemm_kernel<false, 192>;
+    default: return cluster ? igemm_kernel<true, 256> : igemm_kernel<false, 256>;
+  }
+}
+
 int igemm_prepare() {
   static bool seen[16] = {false};
   if (first_use_on_device(seen)) {
-    TDX_CHECK_CUDA(cudaFuncSetAttribute(igemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
-    TDX_CHECK_CUDA(cudaFuncSetAttribute(igemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
+    for (int n = 64; n <= 256; n += 64)
+      for (int cl = 0; cl < 2; ++cl)
+        TDX_CHECK_CUDA(
+            cudaFuncSetAttribute(igemm_kernel_for(cl, n), cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
   }
   float* ws;
   return ensure_scratch(&ws);
@@ -951,8 +919,8 @@ static int max_active_clusters(int csize) {
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   int n = 0;
-  cudaFuncSetAttribute(igemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
-  if (cudaOccupancyMaxActiveClusters(&n, igemm_kernel<true>, &cfg) != cudaSuccess || n <= 0) {
+  cudaFuncSetAttribute(igemm_kernel<true, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
+  if (cudaOccupancyMaxActiveClusters(&n, igemm_kernel<true, 64>, &cfg) != cudaSuccess || n <= 0) {
     cudaGetLastError();
     n = (sm_count() * 3 / 4) / csize;   // no GPU to ask (or the query failed): assume some GPCs cannot be filled
   }
@@ -960,33 +928,36 @@ static int max_active_clusters(int csize) {
   return n;
 }
 
-// Choose the output-channel width of a work item (MMA N) and the split-K factor.  Model (cycles), from measurements
-// on B200:
-//   * an SS-mode M=128 K=16 tcgen05.mma occupies the tensor pipe for max(48, N/2) cycles (tools/probe/mma_probe3.cu; the
-//     86 cycles of round 1 were R2UR-bound issue, not the pipe);
-//   * L2 -> SM delivers ~5 KB/clk chip-wide (tools/sweep_igemm.py) and ~56 B/clk into one SM; per item the A patches (23 KB per 64 input
+// Choose the output-channel width of a work item (MMA N) and the split-K factor.  A rough cost model (cycles):
+//   * the 128 x N x 16 product of one K step takes N cycles of the SM's tensor cores (dense bf16 peak of the H100
+//     data sheet: ~2048 multiply-adds per SM per cycle);
+//   * L2 -> SM delivers ~5 KB/clk chip-wide and ~56 B/clk into one SM; per item the A patches (23 KB per 64 input
 //     channels) and, unless the item's whole weight slice fits the B ring ("resident": loaded once per CTA), the
 //     weights (N*128 B per stage);
+//   * the fp32 staging tile (N * kStgLd * 4 B) shares shared memory with the rings: wide items get shallower rings,
+//     and a one-slot weight ring cannot overlap weight loads with the MMAs;
 //   * layers with fewer work items than SMs are a serial MMA chain per CTA: split their (chunk, tap) stages over the
 //     `ks` CTAs of a cluster, which reduce-scatter fp32 partial sums through L2 (each part then finalises N/ks columns,
 //     so N/ks must be a multiple of the epilogue's 32-column chunk);
 //   * pixel-norm layers exchange statistics inside a cluster, so all nsplit*ks CTAs of an M tile share one (<= 8).
-struct ItemShape { int ncta, resident, sb, ksplit; };
+struct ItemShape { int ncta, resident, sa, sb, ksplit; };
 
 static ItemShape choose_item_shape(int cout, int tiles, int stages, int chunks, int forced_n, bool norm,
                                    int want_k = 0) {
   if (!forced_n && getenv("TDX_IGEMM_N")) forced_n = atoi(getenv("TDX_IGEMM_N"));
   if (forced_n && (forced_n > cout || cout % forced_n)) forced_n = 0;
   const int forced_k = want_k > 0 ? want_k : (getenv("TDX_IGEMM_KSPLIT") ? atoi(getenv("TDX_IGEMM_KSPLIT")) : 0);
-  const int ring_budget = kSmemBudget - kSA * kAStageBytes - kSmemMisc;
   double best = 1e30;
-  ItemShape bs = {64, 0, 2, want_k > 0 ? 0 : 1};   // ksplit 0 = "the requested split is not possible"
+  ItemShape bs = {64, 0, kSA, 2, want_k > 0 ? 0 : 1};   // ksplit 0 = "the requested split is not possible"
   for (int n = 64; n <= 256 && n <= cout; n += 64) {
     if (cout % n) continue;
     if (forced_n && n != forced_n) continue;
     const int nsplit = cout / n;
     if (norm && nsplit > kMaxSplit) continue;   // pixel-norm statistics travel inside one cluster
     const int stage_bytes = n * 128;
+    const int free_bytes = kSmemBudget - kSmemMisc - n * kStgLd * 4;
+    const int sa = free_bytes - kSA * kAStageBytes >= 2 * stage_bytes ? kSA : 2;
+    const int ring_budget = free_bytes - sa * kAStageBytes;
     const long items = (long)tiles * nsplit;
     for (int ks = 1; ks <= 8; ++ks) {
       const int csize = ks * ((norm && nsplit > 1) ? nsplit : 1);
@@ -1001,13 +972,12 @@ static ItemShape choose_item_shape(int cout, int tiles, int stages, int chunks, 
       const int resident = (ks == 1 && stages * stage_bytes <= ring_budget && stages <= kMaxSB) ? 1 : 0;
       int sb = resident ? stages : ring_budget / stage_bytes;
       if (sb > kMaxSB) sb = kMaxSB;
-      if (sb < 2 && !resident) continue;
+      if (sb < 1) continue;
       int grid = items * ks < sm_count() ? (int)(items * ks) : sm_count();
       grid -= grid % (nsplit * ks);
       if (grid <= 0) continue;
       const double rounds = (double)((items * ks + grid - 1) / grid);
-      const double cyc = n / 2.0 > 48.0 ? n / 2.0 : 48.0;
-      const double mma = rounds * my_stages * 4.0 * cyc + 800.0;
+      const double mma = rounds * my_stages * 4.0 * n * (sb < 2 && !resident ? 2.0 : 1.0) + 800.0;
       const double a_bytes = (double)items * ks * my_chunks * kAStageBytes;
       const double b_bytes = resident ? (double)grid * stages * stage_bytes : (double)items * stages * stage_bytes;
       const double red_bytes = ks > 1 ? (double)(ks - 1) / ks * n * 512.0 : 0.0;   // written and read per CTA
@@ -1022,7 +992,7 @@ static ItemShape choose_item_shape(int cout, int tiles, int stages, int chunks, 
       t += epi + red;
       if (want_k > 0 && ks != want_k) continue;
       if (forced_k > 1 && ks == 1) t *= 1e6;   // debug override: take the forced split whenever it is valid
-      if (t < best) { best = t; bs = {n, resident, sb, ks}; }
+      if (t < best) { best = t; bs = {n, resident, sa, sb, ks}; }
     }
   }
   return bs;
@@ -1055,6 +1025,7 @@ int igemm_launch(const TdxIgemmDesc& d, const CUtensorMap* tms, cudaStream_t str
               d.n_per_item);
   p.ncta = shp.ncta;
   p.resident = shp.resident;
+  p.SA = shp.sa;
   p.SB = shp.sb;
   // streaming rings stay stage by stage: a grouped hand-over makes the issuer wait for a group's LAST stage, which
   // costs latency slack exactly where the weight stream is L2-bound (measured: N=128 layers 5-25 % slower)
@@ -1102,7 +1073,7 @@ int igemm_launch(const TdxIgemmDesc& d, const CUtensorMap* tms, cudaStream_t str
     p.dty = dstep % p.tiles_y;
     p.dimg = dstep / p.tiles_y;
   }
-  const int smem = kSA * kAStageBytes + p.SB * p.b_stage_bytes + kSmemMisc;
+  const int smem = p.SA * kAStageBytes + p.SB * p.b_stage_bytes + kSmemMisc + p.ncta * kStgLd * 4;
   const CUtensorMap& t0 = tms[0];
   const CUtensorMap& t1 = tms[d.n_seg > 1 ? 1 : 0];
   const CUtensorMap& t2 = tms[d.n_seg > 2 ? 2 : 0];
@@ -1117,8 +1088,7 @@ int igemm_launch(const TdxIgemmDesc& d, const CUtensorMap* tms, cudaStream_t str
     cfg.attrs = attr;
     cfg.numAttrs += 1;
   }
-  if (cluster > 1 || !TDX_V_TWO_KERNELS) TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, igemm_kernel<true>, t0, t1, t2, p));
-  else TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, igemm_kernel<false>, t0, t1, t2, p));
+  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, igemm_kernel_for(cluster > 1 || !TDX_V_TWO_KERNELS, p.ncta), t0, t1, t2, p));
   return TDX_OK;
 }
 

@@ -1,5 +1,5 @@
 """Unbounded, lazy, device-resident canvas -- the arithmetic and window protocol of the reference's external canvas
-engine (`infinite_tensor>=0.3.0`, requirements.txt:32; absent from /root/reference), as observable from its call sites
+engine (`infinite_tensor>=0.3.0`, requirements.txt:32; absent from the reference checkout), as observable from its call sites
 (world_pipeline.py:982-992,1146-1201,1259-1270; annotated_infinite_panorama.py:141-226; SURVEY.md Appendix C):
 
   * `TensorWindow(size, stride, offset)`: window index k along an axis covers [k*stride+offset, k*stride+offset+size);

@@ -41,7 +41,7 @@ def gaussian_noise_patch(base_seed: int, y0: int, x0: int, h: int, w: int, chann
     """(C, h, w) fp32 CUDA tensor: the patch at integer world origin (y0, x0); negative coordinates supported."""
     dev = torch.device(device)
     if dev.type != "cuda":
-        raise L.TdxError("gaussian_noise_patch (B200 path) generates on the GPU; there is no CPU path")
+        raise L.TdxError("gaussian_noise_patch (GPU path) generates on the GPU; there is no CPU path")
     nbytes = int(L.lib().tdx_noise_patch_workspace_bytes(channels, tile_h, tile_w))
     # one scratch per (device, size, stream): two streams of one device must not share the counts / status words
     key = (dev, nbytes, L.current_stream_ptr(dev))
@@ -63,7 +63,7 @@ def gaussian_noise_patches(base_seed: int, origins, h: int, w: int, channels: in
     import ctypes as C
     dev = torch.device(device)
     if dev.type != "cuda":
-        raise L.TdxError("gaussian_noise_patches (B200 path) generates on the GPU; there is no CPU path")
+        raise L.TdxError("gaussian_noise_patches (GPU path) generates on the GPU; there is no CPU path")
     n = len(origins)
     out = torch.empty((n, channels, h, w), dtype=torch.float32, device=dev)
     if n == 0:
@@ -84,7 +84,7 @@ def standard_normal(seed: int, n: int, device="cuda") -> torch.Tensor:
     """portable_rng.standard_normal(seed, n) as an fp32 CUDA tensor (bit-identical stream)."""
     dev = torch.device(device)
     if dev.type != "cuda":
-        raise L.TdxError("standard_normal (B200 path) generates on the GPU; there is no CPU path")
+        raise L.TdxError("standard_normal (GPU path) generates on the GPU; there is no CPU path")
     out = torch.empty((n,), dtype=torch.float32, device=dev)
     if n == 0:
         return out

@@ -1,7 +1,7 @@
 """WorldPipeline -- drop-in for terrain_diffusion.inference.world_pipeline.WorldPipeline (reference
 inference/world_pipeline.py:287-372 constructor, :541-565 from_pretrained, :567-623 device / to / bind, :690-712 cache and
 context manager, :743-819 seed / SNR / custom conditioning, :961-992 + :1133-1203 + :1244-1270 stage wiring,
-:1367-1384 get) whose three stages run on the B200 kernels of this package and whose canvases live in HBM.
+:1367-1384 get) whose three stages run on the H100 kernels of this package and whose canvases live in HBM.
 
 Callers (`api.py`, `explorer/server.py`, `tiff_export.py`, `world_generator.py`, `latency.py`) only use
 `WorldPipeline.from_pretrained(path, seed=..., latents_batch_size=..., torch_compile=..., dtype=..., caching_strategy=...,
@@ -155,7 +155,7 @@ class WorldPipeline:
                 m.save_pretrained(root / folder)
 
     def _apply_dtype_and_compile(self) -> None:
-        """eval mode; the B200 path computes in bf16 on the tensor cores with fp32 accumulation whatever `dtype` says,
+        """eval mode; the GPU path computes in bf16 on the tensor cores with fp32 accumulation whatever `dtype` says,
         so there is nothing to convert or compile (world_pipeline.py:400-430)."""
         for m in (self.coarse_model, self.base_model, self.decoder_model):
             if m is not None:
@@ -183,7 +183,7 @@ class WorldPipeline:
                                       "window cache is the byte-limited HBM cache (cache_limit)")
         if self.device.type != "cuda":
             from .. import _lib as L
-            raise L.TdxError("WorldPipeline (B200 path) needs its models on a CUDA device before bind(); no CPU path")
+            raise L.TdxError("WorldPipeline (GPU path) needs its models on a CUDA device before bind(); no CPU path")
         self._build_hierarchy()
         if self.torch_compile:
             self._prebuild_programs()

@@ -36,7 +36,7 @@ def _on_arg_device(fn):
 
 def _chk(x: torch.Tensor, name: str) -> torch.Tensor:
     if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 2):
-        raise L.TdxError(f"{name}: expected a CUDA float32 [H, W] tensor (the B200 read-out has no CPU path), got "
+        raise L.TdxError(f"{name}: expected a CUDA float32 [H, W] tensor (the GPU read-out has no CPU path), got "
                          f"{getattr(x, 'device', None)} {getattr(x, 'dtype', None)} {tuple(getattr(x, 'shape', ()))}")
     return x.contiguous()
 

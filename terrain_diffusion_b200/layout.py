@@ -1,4 +1,4 @@
-"""Host-side layout helpers: NC8HW8 activations and packed tcgen05 weight stages (see include/tdx.h)."""
+"""Host-side layout helpers: NC8HW8 activations and packed wgmma weight stages (see include/tdx.h)."""
 from __future__ import annotations
 
 import torch

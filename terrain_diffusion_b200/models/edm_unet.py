@@ -1,5 +1,5 @@
 """EDMUnet2D -- drop-in for terrain_diffusion.models.edm_unet.EDMUnet2D (reference edm_unet.py:15-193) whose forward
-runs on hand-written sm_100a kernels through libtdx (see plan.py for how blocks map to launches).
+runs on hand-written sm_90a kernels through libtdx (see plan.py for how blocks map to launches).
 
 Same constructor arguments, same parameter names/shapes (reference checkpoints load with load_state_dict /
 from_pretrained), same call signature `model(x, noise_labels, conditional_inputs, return_logvar=False,
@@ -229,7 +229,7 @@ class EDMUnet2D(nn.Module):
         if self._folded is None:
             dev = self.device
             if dev.type != "cuda":
-                raise L.TdxError("EDMUnet2D (B200 path) needs its parameters on a CUDA device; there is no CPU path")
+                raise L.TdxError("EDMUnet2D (GPU path) needs its parameters on a CUDA device; there is no CPU path")
             L.lib()
             self._folded = FoldedWeights(self, dev)
         return self._folded
@@ -260,9 +260,9 @@ class EDMUnet2D(nn.Module):
         conditional_inputs = conditional_inputs or []
         assert len(conditional_inputs) == len(self.conditional_layers), "Invalid number of conditional inputs"
         if self.training:
-            raise L.TdxError("the B200 path is inference-only: call model.eval()")
+            raise L.TdxError("the GPU path is inference-only: call model.eval()")
         if x.device.type != "cuda":
-            raise L.TdxError("EDMUnet2D (B200 path) got a CPU tensor; there is no CPU fallback")
+            raise L.TdxError("EDMUnet2D (GPU path) got a CPU tensor; there is no CPU fallback")
         n, c, h, w = x.shape
         needs_host_emb = precomputed_embeds is not None or len(self.conditional_layers) > 0 or \
             not (self.noise_fourier is not None and self.noise_fourier.positional)

@@ -2,7 +2,7 @@
 
 The reference evaluates ~6 500 ATen ops per forward (weight re-normalisation, pixel-norm, mp_silu, mp_sum, mp_concat,
 resample, clip around 96 convolutions).  Here every UNetBlock (models/unet_block.py:116-156) becomes two launches of the
-tcgen05 implicit-GEMM kernel (three for encoder blocks with a 1x1 skip) whose epilogues carry all of that:
+wgmma implicit-GEMM kernel (three for encoder blocks with a 1x1 skip) whose epilogues carry all of that:
 
   enc block   [K1: 1x1 skip -> pixel-norm -> (x_n, mp_silu(x_n))]                         (only if Cin != Cout)
               res0: conv3x3(a) -> mp_silu(y * c)                                          (c = embedding modulation)
@@ -36,7 +36,7 @@ TUNED_PATH = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file
 
 
 def tuned_shapes() -> dict:
-    """{"cout|n|h|w|segments|norm": [n_per_item, k_split]} measured on a B200 (tools/tune_igemm.py)."""
+    """{"cout|n|h|w|segments|norm": [n_per_item, k_split]} measured on the GPU (tools/tune_igemm.py)."""
     global _TUNED
     if _TUNED is None:
         _TUNED = {}
@@ -129,7 +129,7 @@ class FoldedWeights:
         for bad in ("conv_type", "resample_type", "activation", "no_padding", "expansion_factor"):
             if bk.get(bad) not in (None, "default", "pooling", "silu", False, 1):
                 raise NotImplementedError(f"block_kwargs[{bad!r}]={bk[bad]!r} is not used by any shipped model and is "
-                                          "not implemented by the B200 path")
+                                          "not implemented by the GPU path")
         self.t_res = float(bk.get("res_balance", 0.3))
         self.clip = float(bk.get("clip_act", 256.0) or 0.0)
         self.cb = float(cfg.get("concat_balance", 0.3))
@@ -139,7 +139,7 @@ class FoldedWeights:
         for b in enc + dec:
             b["heads"] = (b["cout"] // self.cph) if b.get("attention") else 0
             if b["heads"] and self.cph != 64:
-                raise NotImplementedError(f"attention block {b['name']}: channels_per_head={self.cph}; the B200 path "
+                raise NotImplementedError(f"attention block {b['name']}: channels_per_head={self.cph}; the GPU path "
                                           "implements the shipped value 64")
         self.mc = cfg.get("model_channels", 128)
         mults = cfg.get("model_channel_mults") or [1, 2, 3, 4]
@@ -430,7 +430,7 @@ class UNetEmitter:
 
     def _apply_tuned_shape(self, d):
         """Work-item width N and split-K factor of this launch: from the measured table (tuned_shapes.json, produced on
-        a B200 by tools/tune_igemm.py: the library's cost model is only the fallback), or measured now when
+        the GPU by tools/tune_igemm.py: the library's cost model is only the fallback), or measured now when
         TDX_AUTOTUNE=1.  The table is a file, not a run-time search, so every process / rank makes the same choice and
         multi-GPU results stay bit-identical to single-GPU ones."""
         wkey = getattr(d, "_wkey", None)

@@ -49,7 +49,7 @@ class EDMDPMSolverMultistepScheduler:
             raise NotImplementedError(
                 f"algorithm_type={algorithm_type!r}, solver_type={solver_type!r}, solver_order={solver_order}, "
                 f"thresholding={thresholding}: only dpmsolver++ / midpoint / order<=2 / no thresholding (the shipped "
-                "configuration) is implemented on the B200 path")
+                "configuration) is implemented on the GPU path")
         if prediction_type not in ("epsilon", "v_prediction"):
             raise ValueError(f"Prediction type {prediction_type} is not supported.")
         self._internal_dict = _AttrDict(
@@ -200,7 +200,7 @@ class EDMDPMSolverMultistepScheduler:
             raise ValueError(
                 "Number of inference steps is 'None', you need to run 'set_timesteps' after creating the scheduler")
         if sample.device.type != "cuda":
-            raise L.TdxError("scheduler.step (B200 path) needs CUDA tensors; there is no CPU fallback")
+            raise L.TdxError("scheduler.step (GPU path) needs CUDA tensors; there is no CPU fallback")
         if self._step_index is None:
             self._init_step_index(timestep)
         i = self._step_index

@@ -1,8 +1,8 @@
-"""Generate the golden fixtures in tests/golden/ from the UNMODIFIED reference at /root/reference.
+"""Generate the golden fixtures in tests/golden/ from the UNMODIFIED reference (checkout at $TERRAIN_DIFFUSION_REF).
 
 Run once in the build container (the reference cannot travel to the GPU box):
     python tests/golden/make_golden.py
-Needs: /root/reference, oracle/_stub (diffusers mixin stand-in, no arithmetic), numba.
+Needs: $TERRAIN_DIFFUSION_REF, oracle/_stub (diffusers mixin stand-in, no arithmetic), numba.
 Everything written here is small (inputs/outputs only; weights are re-created procedurally from names + seed by
 oracle.unet.procedural_state_dict, identically here and in the tests).
 """
@@ -18,7 +18,7 @@ import torch
 
 HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent.parent
-REF = Path("/root/reference")
+REF = Path(os.environ["TERRAIN_DIFFUSION_REF"])   # a checkout of the original terrain-diffusion project
 sys.path[:0] = [str(ROOT / "oracle" / "_stub"), str(REF), str(ROOT)]
 
 from terrain_diffusion.inference import portable_rng as ref_rng  # noqa: E402

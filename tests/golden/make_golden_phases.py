@@ -4,6 +4,7 @@ ast and compiled unchanged) on the demo's DDIM-style timesteps and on an EDM-sch
 
     python tests/golden/make_golden_phases.py     ->  tests/golden/phases_golden.npz
 """
+import os
 import ast
 import sys
 from pathlib import Path
@@ -13,7 +14,7 @@ import torch
 
 HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent.parent
-REF = Path("/root/reference")
+REF = Path(os.environ["TERRAIN_DIFFUSION_REF"])   # a checkout of the original terrain-diffusion project
 sys.path[:0] = [str(ROOT / "oracle" / "_stub"), str(REF), str(ROOT)]
 from terrain_diffusion.scheduler.dpmsolver import EDMDPMSolverMultistepScheduler  # noqa: E402
 

@@ -8,6 +8,8 @@ Only outputs are stored (tests/golden/post_golden.npz); inputs are regenerated f
 """
 from __future__ import annotations
 
+import os
+
 import ast
 import sys
 from pathlib import Path
@@ -18,7 +20,7 @@ import torch
 
 HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent.parent
-REF = Path("/root/reference")
+REF = Path(os.environ["TERRAIN_DIFFUSION_REF"])   # a checkout of the original terrain-diffusion project
 sys.path[:0] = [str(ROOT / "oracle" / "_stub"), str(REF), str(ROOT)]
 
 from terrain_diffusion.data.laplacian_encoder import laplacian_decode, laplacian_denoise  # noqa: E402

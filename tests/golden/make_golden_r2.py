@@ -1,5 +1,5 @@
 """Round-2 golden fixtures (tests/golden/parity_r2_golden.npz), generated in the build container from the UNMODIFIED
-reference at /root/reference (it cannot travel to the GPU box):
+reference (checkout at $TERRAIN_DIFFUSION_REF; the GPU tests only read the stored result):
 
   ref_bf16_err_{64,128,256}   rel-RMS of the reference's OWN bf16 mode (model.to(bfloat16), bf16 input -- what
                               WorldPipeline does for dtype='bf16', world_pipeline.py:414-419) against its fp32 output on
@@ -17,6 +17,8 @@ Inputs are torch.Generator streams (seeds below) so the tests re-create them bit
 """
 from __future__ import annotations
 
+import os
+
 import sys
 import time
 from pathlib import Path
@@ -26,7 +28,7 @@ import torch
 
 HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent.parent
-REF = Path("/root/reference")
+REF = Path(os.environ["TERRAIN_DIFFUSION_REF"])   # a checkout of the original terrain-diffusion project
 sys.path[:0] = [str(ROOT / "oracle" / "_stub"), str(REF), str(ROOT)]
 
 from terrain_diffusion.models.edm_unet import EDMUnet2D  # noqa: E402

@@ -11,6 +11,8 @@ with procedural weights.  Nothing from the reference is copied into the repo; on
 """
 from __future__ import annotations
 
+import os
+
 import ast
 import functools
 import sys
@@ -22,7 +24,7 @@ import torch
 
 HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent.parent
-REF = Path("/root/reference")
+REF = Path(os.environ["TERRAIN_DIFFUSION_REF"])   # a checkout of the original terrain-diffusion project
 sys.path[:0] = [str(ROOT / "oracle" / "_stub"), str(REF), str(ROOT)]
 
 from terrain_diffusion.inference import portable_rng as ref_rng  # noqa: E402

@@ -32,8 +32,8 @@ def test_gpu_arms_are_declared():
 
 
 def test_committed_headline_line_carries_every_contract_key():
-    """The bench line kept under profiles/ (the closing run of the round) has the keys the driver's contract names."""
-    d = json.loads((ROOT / "profiles" / "r02_bench_tiles1.json").read_text())
+    """The bench line kept under profiles/ (an H100 run of the default workload) has every key of the result line."""
+    d = json.loads((ROOT / "profiles" / "bench_tiles1.json").read_text())
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling",
               "vs_baseline", "dtype", "data", "config", "clocks", "e2e", "gpu_launches", "roofline", "cpu_baseline"):
         assert k in d, k

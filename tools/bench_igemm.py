@@ -1,6 +1,6 @@
-"""Micro-benchmark of the tcgen05 implicit-GEMM conv on the decoder's layer shapes (CUDA events, L2 flushed).
+"""Micro-benchmark of the wgmma implicit-GEMM conv on the decoder's layer shapes (CUDA events, L2 flushed).
 
-Run on the GPU box:  python tools/bench_igemm.py [--batch N]   -> gpurun_out/bench_igemm.txt
+Run on the GPU box:  python tools/bench_igemm.py [--batch N]   -> tool_out/bench_igemm.txt
 """
 from __future__ import annotations
 
@@ -81,8 +81,8 @@ def main():
     s = f"weighted: {tot_t:.3f} ms per forward-equivalent, {tot_f/tot_t/1e9:.1f} TFLOP/s"
     print(s)
     lines.append(s)
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open(f"gpurun_out/bench_igemm_b{args.batch}.txt", "w") as f:
+    os.makedirs("tool_out", exist_ok=True)
+    with open(f"tool_out/bench_igemm_b{args.batch}.txt", "w") as f:
         f.write("\n".join(lines) + "\n")
 
 

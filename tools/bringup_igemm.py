@@ -1,7 +1,7 @@
-"""GPU bring-up of the tcgen05 implicit-GEMM conv: runs every case of tests/_igemm_ref.py, prints error statistics and,
+"""GPU bring-up of the wgmma implicit-GEMM conv: runs every case of tests/_igemm_ref.py, prints error statistics and,
 on failure, a breakdown (by tile row/column, channel group, tap) that localises descriptor/layout mistakes.
 
-Run on the GPU box:  python tools/bringup_igemm.py  (writes gpurun_out/bringup_igemm.txt as well)
+Run on the GPU box:  python tools/bringup_igemm.py  (writes tool_out/bringup_igemm.txt as well)
 """
 from __future__ import annotations
 
@@ -115,8 +115,8 @@ def main():
             if "CUDA" in traceback.format_exc() or "cuda" in traceback.format_exc():
                 break
     log("FAILURES:", n_fail)
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/bringup_igemm.txt", "w") as f:
+    os.makedirs("tool_out", exist_ok=True)
+    with open("tool_out/bringup_igemm.txt", "w") as f:
         f.write("\n".join(LOG) + "\n")
     return 1 if n_fail else 0
 

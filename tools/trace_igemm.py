@@ -1,8 +1,7 @@
 """Per-tile phase timeline of CTA 0 of the igemm kernel (debug hook tdx_debug_set_igemm_trace).
 
     python tools/trace_igemm.py [flags]      # flags = OR of the kernel's ablation bits (tdx_debug_set_igemm_flags):
-        1  A descriptors with SBO=128 (wrong results; smem bank-conflict experiment)     2  no weight loads
-        4  epilogue does nothing      8  no epilogue warps      16  compute everything, store nothing
+        2  no weight loads      4  epilogue does nothing      16  compute everything, store nothing
         32 skip the residual pixel-norm pre-pass      64 only output 0 is produced
     python tools/trace_igemm.py floor        # launch floor of an empty-ish kernel
 """
@@ -24,8 +23,7 @@ from terrain_diffusion_b200.layout import pack_weight_segments, to_nc8hw8
 
 SHAPES = [("64->64 1x1 @16 (tiny)", [(64, 1)], 64, 16), ("64->64 @128 (<=2 items/CTA)", [(64, 9)], 64, 128), ("64->64 @256", [(64, 9)], 64, 256), ("128->128 @128", [(128, 9)], 128, 128),
           ("256->256 @32", [(256, 9)], 256, 32), ("192->192 @64", [(192, 9)], 192, 64)]
-NAMES = ["A-prod start", "mma: tmem free", "mma: A landed", "mma: issued+commit", "epi: waiting", "epi: acc ready",
-         "epi: done"]
+NAMES = ["A-prod start", "mma: start", "mma: acc staged", "split-K: partials published", "epi: done"]
 
 
 def main():
@@ -68,7 +66,7 @@ def main():
         t0 = t[127]
         print(f"== {name}: clocks relative to CTA-0 setup done; kernel entry at {t[126]-t0}, exit at {t[125]-t0}")
         for it in range(4):
-            row = t[it * 8: it * 8 + 7]
+            row = t[it * 8: it * 8 + len(NAMES)]
             if row[0] == 0 and row[1] == 0:
                 break
             print(f"  tile {it}: " + "  ".join(f"{n}={v - t0 if v else -1}" for n, v in zip(NAMES, row)))

@@ -1,13 +1,13 @@
 """Measure the best (n_per_item, k_split) of every implicit-GEMM launch shape of the shipped models on THIS GPU and
 write terrain_diffusion_b200/tuned_shapes.json (the planner's lookup table; the library's cost model is the fallback).
 
-    python tools/tune_igemm.py [decoder|coarse|base ...]      # on a B200 (gpurun); merges into the existing table
+    python tools/tune_igemm.py [decoder|coarse|base ...]      # on the GPU; merges into the existing table
 
 Method ("in the graph"): for one (model, batch, size) the whole forward is planned and replayed as its CUDA graph; then,
 shape by shape in program order, every valid (N, k_split) of that shape is tried -- the forward is re-planned with the
 candidate and the graph replay is timed (median of 3 x 20 replays) -- and the fastest is kept (coordinate descent, one
 pass).  Timing the layer inside the real forward matters: back-to-back launches of one layer keep its weights and inputs
-hot in L2 and favour weight-streaming shapes that lose inside the forward (profiles/r02_tuning_notes.txt).
+hot in L2 and favour weight-streaming shapes that lose inside the forward.
 """
 import json
 import os
