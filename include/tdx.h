@@ -37,7 +37,7 @@ extern "C" {
 const char* tdx_last_error(void);
 /* Library + device probe: fills sm count, compute capability; fails if the device is not sm_90. */
 int tdx_device_info(int* sm_count, int* cc_major, int* cc_minor);
-/* sizeof() of the public structs (0: TdxOutSpec, 1: TdxIgemmDesc, 2: TdxConvInDesc, 3: TdxConvOutDesc, 4: TdxEmbedBlock, 5: TdxEmbedDesc, 6: TdxAttnDesc) so bindings can verify their layout. */
+/* sizeof() of the public structs (0: TdxOutSpec, 1: TdxIgemmDesc, 2: TdxConvOutDesc, 3: TdxEmbedBlock, 4: TdxEmbedDesc, 5: TdxAttnDesc, 6: TdxIm2colDesc) so bindings can verify their layout. */
 int tdx_abi_sizeof(int which);
 
 /* ------------------------------------------------------------------------------------------------------------------
@@ -87,11 +87,6 @@ typedef struct TdxIgemmDesc {
    * the residual to recompute it.  Both may be NULL. */
   float* rms_out;
   const float* resid_inv;
-  /* Split-K factor: 0 = the library's cost model picks it (together with the residency of the weights); > 0 forces it
-   * (the launch fails with TDX_E_INVALID when that split is impossible for the shape).  Used with n_per_item by the
-   * measured per-shape table terrain_diffusion_b200/tuned_shapes.json (tools/tune_igemm.py). */
-  int32_t k_split;
-  int32_t _reserved;
 } TdxIgemmDesc;
 
 /* Output channels per work item (64/128/192/256) the library prefers for this launch shape: balances the MMA issue
@@ -105,34 +100,21 @@ int tdx_igemm_run(const TdxIgemmDesc* desc, void* stream);
 
 
 /* ------------------------------------------------------------------------------------------------------------------
- * First convolution (EDMUnet2D.forward, models/edm_unet.py:168-172: cat([x, ones]) -> enc['..._conv'] = MPConv 3x3).
- * Reads the caller's planar NCHW input directly (up to two sources, e.g. the scaled noisy sample and the conditioning
- * image of sample_decoder_diffusion_tiled, training/evaluation/sample_diffusion_decoder.py:108-110), appends the
- * ones channel (zero-padded at the border like the reference's conv), and writes bf16 NC8HW8 outputs.
+ * First convolution (EDMUnet2D.forward, models/edm_unet.py:168-172: cat([x, ones]) -> enc['..._conv'] = MPConv 3x3)
+ * on the tensor cores.  Reads the caller's planar NCHW input directly (up to two sources, e.g. the scaled noisy sample
+ * and the conditioning image of sample_decoder_diffusion_tiled, training/evaluation/sample_diffusion_decoder.py:
+ * 108-110).  This launch only gathers the 3x3 neighbourhood of every pixel into a bf16 NC8HW8 tensor of k_pad
+ * "channels" -- channel k = tap * ci + c for tap = 3*dy+dx in 0..8 and c in 0..ci-1 (ci = sum(src_channels) + 1, the
+ * ones channel last; zero outside the image, like the reference's padded conv), zero for k >= 9*ci -- and the
+ * convolution itself becomes a 1x1 tdx_igemm_run over that tensor with the weight matrix [c_out][k_pad] (so it gets
+ * the igemm epilogue: pixel-norm, silu, three outputs).  The inputs and weights are rounded to bf16, as in the
+ * reference's bf16 autocast of models/edm_unet.py:168-172.
  * ------------------------------------------------------------------------------------------------------------------ */
-typedef struct TdxConvInDesc {
-  const void* src[2];        /* NCHW planar, n_img x src_channels[i] x H x W */
-  int32_t src_channels[2];   /* channels of each source (second may be 0) */
-  int32_t src_dtype[2];      /* 0 = fp32, 1 = bf16 */
-  const float* src_scale[2]; /* optional DEVICE scalar multiplied into source i (precondition_inputs), or NULL */
-  const float* weight;       /* fp32 effective weights, tap-major [3*3][sum(src_channels)+1][c_out] (ones channel last) */
-  int32_t c_out;             /* multiple of 64, <= 256; sum(src_channels) <= 15 */
-  int32_t n_img, height, width;
-  TdxOutSpec out[3];         /* same semantics as TdxIgemmDesc.out (TDX_SP_SAME only) */
-} TdxConvInDesc;
-int tdx_conv_in_run(const TdxConvInDesc* desc, void* stream);
-
-/* The same first convolution on the tensor cores: this launch only gathers the 3x3 neighbourhood of every pixel into
- * a bf16 NC8HW8 tensor of k_pad "channels" -- channel k = tap * ci + c for tap = 3*dy+dx in 0..8 and c in
- * 0..ci-1 (ci = sum(src_channels) + 1, the ones channel last; zero outside the image, like the reference's padded
- * conv), zero for k >= 9*ci -- and the convolution itself becomes a 1x1 tdx_igemm_run over that tensor with the
- * weight matrix [c_out][k_pad] (so it gets the igemm epilogue: pixel-norm, silu, three outputs).  The inputs and
- * weights are rounded to bf16, as in the reference's bf16 autocast of models/edm_unet.py:168-172. */
 typedef struct TdxIm2colDesc {
   const void* src[2];        /* NCHW planar, n_img x src_channels[i] x H x W */
   int32_t src_channels[2];   /* channels of each source (second may be 0) */
   int32_t src_dtype[2];      /* 0 = fp32, 1 = bf16 */
-  const float* src_scale[2]; /* optional DEVICE scalar multiplied into source i, or NULL */
+  const float* src_scale[2]; /* optional DEVICE scalar multiplied into source i (precondition_inputs), or NULL */
   void* out;                 /* bf16 NC8HW8 [n_img][k_pad/8][H][W][8] */
   int32_t k_pad;             /* 9 * (sum(src_channels) + 1) rounded up to a multiple of 64; sum = 5 or 11 */
   int32_t n_img, height, width;
@@ -300,7 +282,6 @@ uint64_t tdx_tile_seed(uint64_t base_seed, int64_t ty, int64_t tx);
  * ------------------------------------------------------------------------------------------------------------------ */
 typedef struct TdxProgram TdxProgram;
 int tdx_program_create(TdxProgram** out);
-int tdx_program_add_conv_in(TdxProgram* p, const TdxConvInDesc* d);
 int tdx_program_add_im2col(TdxProgram* p, const TdxIm2colDesc* d);
 int tdx_program_add_igemm(TdxProgram* p, const TdxIgemmDesc* d);
 int tdx_program_add_conv_out(TdxProgram* p, const TdxConvOutDesc* d);
@@ -312,7 +293,7 @@ int tdx_program_run(TdxProgram* p, int use_graph, void* stream);
 /* Capture + instantiate + upload the graph without running it (keeps one-time costs out of timed regions). */
 int tdx_program_instantiate(TdxProgram* p, void* stream);
 /* Eager run with a CUDA event pair around every launch: ms_per_launch[i] = device time of launch i (in program
- * order, tdx_program_num_launches entries); kinds[i] = 0 conv_in, 1 igemm, 2 conv_out, 3 embed, 4 attn, 5 im2col.  Synchronises. */
+ * order, tdx_program_num_launches entries); kinds[i] = 1 igemm, 2 conv_out, 3 embed, 4 attn, 5 im2col.  Synchronises. */
 int tdx_program_profile(TdxProgram* p, float* ms_per_launch, int32_t* kinds, void* stream);
 int tdx_program_destroy(TdxProgram* p);
 

@@ -24,15 +24,6 @@ class TdxIgemmDesc(C.Structure):
         ("height", C.c_int32), ("width", C.c_int32), ("epi_flags", C.c_int32), ("cvec", C.c_void_p), ("resid", C.c_void_p),
         ("resid_spatial", C.c_int32), ("resid_pnorm", C.c_int32), ("resid_scale", C.c_float), ("clip", C.c_float),
         ("out", TdxOutSpec * 3), ("rms_out", C.c_void_p), ("resid_inv", C.c_void_p),
-        ("k_split", C.c_int32), ("_reserved", C.c_int32),
-    ]
-
-
-class TdxConvInDesc(C.Structure):
-    _fields_ = [
-        ("src", C.c_void_p * 2), ("src_channels", C.c_int32 * 2), ("src_dtype", C.c_int32 * 2),
-        ("src_scale", C.c_void_p * 2), ("weight", C.c_void_p), ("c_out", C.c_int32), ("n_img", C.c_int32),
-        ("height", C.c_int32), ("width", C.c_int32), ("out", TdxOutSpec * 3),
     ]
 
 
@@ -69,8 +60,7 @@ class TdxAttnDesc(C.Structure):
                 ("heads", C.c_int32), ("head_dim", C.c_int32), ("tokens", C.c_int32)]
 
 
-ABI_STRUCTS = [TdxOutSpec, TdxIgemmDesc, TdxConvInDesc, TdxConvOutDesc, TdxEmbedBlock, TdxEmbedDesc, TdxAttnDesc,
-               TdxIm2colDesc]
+ABI_STRUCTS = [TdxOutSpec, TdxIgemmDesc, TdxConvOutDesc, TdxEmbedBlock, TdxEmbedDesc, TdxAttnDesc, TdxIm2colDesc]
 
 OUT_NONE, OUT_RAW, OUT_SILU, OUT_PNORM_SILU = 0, 1, 2, 3
 SP_SAME, SP_DOWN2, SP_UP2 = 0, 1, 2
@@ -108,9 +98,8 @@ def _declare(l: C.CDLL) -> None:
     for i, st in enumerate(ABI_STRUCTS):
         if l.tdx_abi_sizeof(i) != C.sizeof(st):
             raise TdxError(f"ABI mismatch for {st.__name__}: C {l.tdx_abi_sizeof(i)} vs ctypes {C.sizeof(st)}")
-    for name, desc in (("tdx_conv_in_run", TdxConvInDesc), ("tdx_conv_out_run", TdxConvOutDesc),
-                       ("tdx_embed_run", TdxEmbedDesc), ("tdx_attn_run", TdxAttnDesc),
-                       ("tdx_im2col_run", TdxIm2colDesc)):
+    for name, desc in (("tdx_conv_out_run", TdxConvOutDesc), ("tdx_embed_run", TdxEmbedDesc),
+                       ("tdx_attn_run", TdxAttnDesc), ("tdx_im2col_run", TdxIm2colDesc)):
         fn = getattr(l, name)
         fn.restype = C.c_int
         fn.argtypes = [C.POINTER(desc), C.c_void_p]
@@ -172,9 +161,9 @@ def _declare(l: C.CDLL) -> None:
     l.tdx_tile_seed.argtypes = [C.c_uint64, C.c_int64, C.c_int64]
     l.tdx_program_create.restype = C.c_int
     l.tdx_program_create.argtypes = [C.POINTER(C.c_void_p)]
-    for name, desc in (("tdx_program_add_conv_in", TdxConvInDesc), ("tdx_program_add_igemm", TdxIgemmDesc),
-                       ("tdx_program_add_conv_out", TdxConvOutDesc), ("tdx_program_add_embed", TdxEmbedDesc),
-                       ("tdx_program_add_attn", TdxAttnDesc), ("tdx_program_add_im2col", TdxIm2colDesc)):
+    for name, desc in (("tdx_program_add_igemm", TdxIgemmDesc), ("tdx_program_add_conv_out", TdxConvOutDesc),
+                       ("tdx_program_add_embed", TdxEmbedDesc), ("tdx_program_add_attn", TdxAttnDesc),
+                       ("tdx_program_add_im2col", TdxIm2colDesc)):
         fn = getattr(l, name)
         fn.restype = C.c_int
         fn.argtypes = [C.c_void_p, C.POINTER(desc)]

@@ -25,12 +25,8 @@ NVCC_FLAGS = [
 ]
 
 
-if os.environ.get("TDX_DEBUG_HOOKS") == "1":      # ablation flags / trace clocks / launch timeline for tools/trace_igemm.py etc.
+if os.environ.get("TDX_DEBUG_HOOKS") == "1":      # trace clocks / launch timeline for tools/trace_igemm.py etc.
     NVCC_FLAGS.append("-DTDX_DEBUG_HOOKS=1")
-
-
-for _flag in os.environ.get("TDX_NVCC_DEFINES", "").split():     # A/B experiments: TDX_NVCC_DEFINES="TDX_V_AHEAD_R=0 TDX_EPI_CHUNK=16 ..."
-    NVCC_FLAGS.append("-D" + _flag)
 
 
 def _sources() -> list[Path]:
@@ -52,7 +48,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     if not force and LIB.exists() and STAMP.exists() and STAMP.read_text().strip() == digest:
         return LIB
     nvcc = os.environ.get("NVCC", "nvcc")
-    cmd = [nvcc, *NVCC_FLAGS, "-o", str(LIB), *map(str, _sources()), "-lcuda" if False else "-ldl"]
+    cmd = [nvcc, *NVCC_FLAGS, "-o", str(LIB), *map(str, _sources()), "-ldl"]
     if verbose:
         cmd.insert(1, "-Xptxas")
         cmd.insert(2, "-v")

@@ -2,7 +2,6 @@
 #include "tdx_common.h"
 
 #include <cudaTypedefs.h>
-#include <stdlib.h>
 #include <string.h>
 
 namespace tdx {
@@ -40,15 +39,6 @@ bool first_use_on_device(bool (&seen)[16]) {
   return true;
 }
 
-static bool use_pdl() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("TDX_PDL");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-
 void fill_launch_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, dim3 grid, dim3 block, size_t smem,
                         cudaStream_t stream) {
   memset(cfg, 0, sizeof(*cfg));
@@ -56,12 +46,10 @@ void fill_launch_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, dim3
   cfg->blockDim = block;
   cfg->dynamicSmemBytes = smem;
   cfg->stream = stream;
-  if (use_pdl()) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg->attrs = attr;
-    cfg->numAttrs = 1;
-  }
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg->attrs = attr;
+  cfg->numAttrs = 1;
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -128,12 +116,11 @@ extern "C" int tdx_abi_sizeof(int which) {
   switch (which) {
     case 0: return (int)sizeof(TdxOutSpec);
     case 1: return (int)sizeof(TdxIgemmDesc);
-    case 2: return (int)sizeof(TdxConvInDesc);
-    case 3: return (int)sizeof(TdxConvOutDesc);
-    case 4: return (int)sizeof(TdxEmbedBlock);
-    case 5: return (int)sizeof(TdxEmbedDesc);
-    case 6: return (int)sizeof(TdxAttnDesc);
-    case 7: return (int)sizeof(TdxIm2colDesc);
+    case 2: return (int)sizeof(TdxConvOutDesc);
+    case 3: return (int)sizeof(TdxEmbedBlock);
+    case 4: return (int)sizeof(TdxEmbedDesc);
+    case 5: return (int)sizeof(TdxAttnDesc);
+    case 6: return (int)sizeof(TdxIm2colDesc);
     default: return -1;
   }
 }

@@ -30,10 +30,10 @@ int sm_count();
     }                                     \
   } while (0)
 
-// Launch configuration with programmatic dependent launch (PDL) enabled unless TDX_PDL=0: every libtdx kernel calls
+bool first_use_on_device(bool (&seen)[16]);
+// Launch configuration with programmatic dependent launch (PDL) enabled: every libtdx kernel calls
 // griddepcontrol.wait before touching data produced by earlier kernels, so consecutive launches may overlap their
 // prologue (barrier init, weight prefetch) with the previous kernel's tail.
-bool first_use_on_device(bool (&seen)[16]);
 void fill_launch_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, dim3 grid, dim3 block, size_t smem,
                         cudaStream_t stream);
 

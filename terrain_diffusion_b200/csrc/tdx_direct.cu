@@ -1,5 +1,5 @@
-// CUDA-core kernels around the tensor-core path: first / last convolution (tiny K or tiny N), the embedding /
-// modulation vectors, and the fp32 elementwise scheduler + blend kernels.  All HBM-bound or launch-bound; the design
+// CUDA-core kernels around the tensor-core path: the first convolution's im2col gather, the last convolution (tiny
+// N), the embedding / modulation vectors, and the fp32 elementwise scheduler + blend kernels.  All HBM-bound or launch-bound; the design
 // rules that matter are coalescing (threads walk x), 16-byte vectors on the NC8HW8 side and broadcast smem weights.
 #include "tdx_common.h"
 #include "tdx_ptx.cuh"
@@ -7,212 +7,6 @@
 namespace tdx {
 
 __device__ __forceinline__ float mp_silu_precise(float x) { return x / (1.0f + expf(-x)) / 0.596f; }
-
-// ------------------------------------------------------------------------------------------------ first conv
-constexpr int kConvInGroups = 4;   // 32-pixel groups per block (amortises the weight staging)
-constexpr int kConvOutGroups = 1;  // conv_out stages only 9*C*COUT weights: more, smaller blocks keep every SM busy
-
-struct ConvInParams {
-  const void* src[2];
-  int src_ch[2];
-  int src_dtype[2];
-  const float* src_scale[2];
-  const float* weight;
-  int ci;  // total input channels incl. the ones channel
-  int cout;
-  int H, W;
-  TdxOutSpec out[3];
-};
-
-__device__ __forceinline__ float load_in(const void* base, int dtype, size_t idx) {
-  if (dtype == 0) return __ldg(reinterpret_cast<const float*>(base) + idx);
-  return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(base)[idx]);
-}
-
-// Block = 128 threads = 32 consecutive pixels x 4 warps; warp w computes output channels [oc0 + 16w, oc0 + 16w + 16)
-// of each 64-channel group, so weights are warp-broadcast shared-memory reads and every store is a 512-byte row of
-// 16-byte pixel vectors.
-template <int CI>
-__global__ void __launch_bounds__(128) conv_in_kernel(const ConvInParams p) {
-  extern __shared__ float ws[];  // [tap][ci][cout]
-  __shared__ float ssq[4][32];
-  const int CO = p.cout;
-  for (int i = threadIdx.x; i < (9 * CI * CO) / 4; i += blockDim.x)
-    reinterpret_cast<float4*>(ws)[i] = __ldg(reinterpret_cast<const float4*>(p.weight) + i);
-  pdl_launch_dependents();
-  pdl_wait();  // the sources / scale come from earlier kernels; weights above are constants
-  __syncthreads();
-  const int img = blockIdx.y;
-  const int lane = threadIdx.x & 31, wq = threadIdx.x >> 5;
-  for (int grp = 0; grp < kConvInGroups; ++grp) {
-  const int pix = (blockIdx.x * kConvInGroups + grp) * 32 + lane;
-  const bool inb = pix < p.H * p.W;
-  const int y = inb ? pix / p.W : 0, x = inb ? pix % p.W : 0;
-  const size_t plane = (size_t)p.H * p.W;
-  const float s0 = p.src_scale[0] ? __ldg(p.src_scale[0]) : 1.0f;
-  const float s1 = p.src_scale[1] ? __ldg(p.src_scale[1]) : 1.0f;
-  const int c0n = p.src_ch[0], c1n = p.src_ch[1];
-  const int C8 = CO >> 3;
-
-  float sumsq = 0.f;
-  for (int oc0 = 0; oc0 < CO; oc0 += 64) {
-    const int oc = oc0 + wq * 16;
-    float acc[16];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) acc[j] = 0.f;
-#pragma unroll 1
-    for (int tap = 0; tap < 9; ++tap) {
-      // the CI input values of this tap (zero padded at the border, ones channel included), loaded as one batch
-      const int yy = y + tap / 3 - 1, xx = x + tap % 3 - 1;
-      const bool ok = inb && yy >= 0 && yy < p.H && xx >= 0 && xx < p.W;
-      const size_t off = (size_t)yy * p.W + xx;
-      float in[CI];
-#pragma unroll
-      for (int ci = 0; ci < CI; ++ci) {
-        float v = 0.f;
-        if (ok) {
-          if (ci < c0n) v = load_in(p.src[0], p.src_dtype[0], ((size_t)img * c0n + ci) * plane + off) * s0;
-          else if (ci < c0n + c1n) v = load_in(p.src[1], p.src_dtype[1], ((size_t)img * c1n + (ci - c0n)) * plane + off) * s1;
-          else v = 1.0f;
-        }
-        in[ci] = v;
-      }
-#pragma unroll
-      for (int ci = 0; ci < CI; ++ci) {
-        {
-          const float v = in[ci];
-          const float4* w4 = reinterpret_cast<const float4*>(ws + (tap * CI + ci) * CO + oc);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float4 w = w4[j];
-            acc[4 * j + 0] = fmaf(w.x, v, acc[4 * j + 0]);
-            acc[4 * j + 1] = fmaf(w.y, v, acc[4 * j + 1]);
-            acc[4 * j + 2] = fmaf(w.z, v, acc[4 * j + 2]);
-            acc[4 * j + 3] = fmaf(w.w, v, acc[4 * j + 3]);
-          }
-        }
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < 16; ++j) sumsq = fmaf(acc[j], acc[j], sumsq);
-    if (inb) {
-#pragma unroll
-      for (int o = 0; o < 3; ++o) {
-        const TdxOutSpec& os = p.out[o];
-        if (os.kind != TDX_OUT_RAW && os.kind != TDX_OUT_SILU) continue;
-        uint4* optr = reinterpret_cast<uint4*>(os.ptr) + ((size_t)img * C8 + (oc >> 3)) * plane + pix;
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          float w[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float t = acc[g * 8 + i];
-            w[i] = os.kind == TDX_OUT_RAW ? t : mp_silu_f(t * os.scale);
-          }
-          uint4 u;
-          u.x = pack_bf16x2(w[0], w[1]); u.y = pack_bf16x2(w[2], w[3]);
-          u.z = pack_bf16x2(w[4], w[5]); u.w = pack_bf16x2(w[6], w[7]);
-          optr[(size_t)g * plane] = u;
-        }
-      }
-    }
-  }
-  bool want_pnorm = false;
-  const uint4* raw_ptr = nullptr;
-#pragma unroll
-  for (int o = 0; o < 3; ++o) {
-    if (p.out[o].kind == TDX_OUT_PNORM_SILU) want_pnorm = true;
-    if (p.out[o].kind == TDX_OUT_RAW) raw_ptr = reinterpret_cast<const uint4*>(p.out[o].ptr);
-  }
-  if (want_pnorm) {
-    // per-pixel sum of squares over all channels = sum over the 4 warps; then re-read this warp's own raw outputs
-    ssq[wq][lane] = sumsq;
-    __syncthreads();
-    const float tot = ssq[0][lane] + ssq[1][lane] + ssq[2][lane] + ssq[3][lane];
-    const float inv = 1.0f / (1e-4f + sqrtf(tot / (float)CO));
-    if (inb) {
-#pragma unroll
-      for (int o = 0; o < 3; ++o) {
-        const TdxOutSpec& os = p.out[o];
-        if (os.kind != TDX_OUT_PNORM_SILU) continue;
-        for (int oc0 = 0; oc0 < CO; oc0 += 64) {
-#pragma unroll
-          for (int g = 0; g < 2; ++g) {
-            const size_t idx = ((size_t)img * C8 + ((oc0 + wq * 16) >> 3) + g) * plane + pix;
-            const uint4 u = raw_ptr[idx];
-            float a[8];
-            unpack_bf16x2(u.x, a[0], a[1]); unpack_bf16x2(u.y, a[2], a[3]);
-            unpack_bf16x2(u.z, a[4], a[5]); unpack_bf16x2(u.w, a[6], a[7]);
-            uint4 r;
-            r.x = pack_bf16x2(mp_silu_f(a[0] * inv), mp_silu_f(a[1] * inv));
-            r.y = pack_bf16x2(mp_silu_f(a[2] * inv), mp_silu_f(a[3] * inv));
-            r.z = pack_bf16x2(mp_silu_f(a[4] * inv), mp_silu_f(a[5] * inv));
-            r.w = pack_bf16x2(mp_silu_f(a[6] * inv), mp_silu_f(a[7] * inv));
-            reinterpret_cast<uint4*>(os.ptr)[idx] = r;
-          }
-        }
-      }
-    }
-  }
-  __syncthreads();  // ssq is reused by the next pixel group
-  }
-}
-
-int direct_prepare();
-
-int conv_in_validate(const TdxConvInDesc& d) {
-  TDX_REQUIRE(d.src[0] && d.src_channels[0] > 0, "conv_in: src[0] missing");
-  TDX_REQUIRE(d.src_channels[1] == 0 || d.src[1], "conv_in: src[1] missing");
-  TDX_REQUIRE(d.weight, "conv_in: weight is null");
-  TDX_REQUIRE(d.c_out >= 64 && d.c_out <= 256 && d.c_out % 64 == 0, "conv_in: c_out=%d (multiple of 64)", d.c_out);
-  TDX_REQUIRE(d.src_channels[0] + d.src_channels[1] + 1 == 6 || d.src_channels[0] + d.src_channels[1] + 1 == 12,
-              "conv_in: %d input channels; instantiated for 5 (decoder / latent models) or 11 (coarse model)",
-              d.src_channels[0] + d.src_channels[1]);
-  TDX_REQUIRE(d.n_img >= 1 && d.height >= 1 && d.width >= 1, "conv_in: bad shape");
-  const int ci = d.src_channels[0] + d.src_channels[1] + 1;
-  TDX_REQUIRE(9 * ci * d.c_out * 4 <= 200 * 1024, "conv_in: weights (%d in, %d out) exceed shared memory", ci, d.c_out);
-  bool has_raw = false, has_pn = false;
-  for (int o = 0; o < 3; ++o) {
-    if (d.out[o].kind == TDX_OUT_NONE) continue;
-    TDX_REQUIRE(d.out[o].ptr, "conv_in: out[%d].ptr is null", o);
-    TDX_REQUIRE(d.out[o].spatial == TDX_SP_SAME, "conv_in: only TDX_SP_SAME outputs");
-    has_raw |= d.out[o].kind == TDX_OUT_RAW;
-    has_pn |= d.out[o].kind == TDX_OUT_PNORM_SILU;
-  }
-  TDX_REQUIRE(!has_pn || has_raw, "conv_in: a PNORM_SILU output needs a RAW output too");
-  return TDX_OK;
-}
-
-int conv_in_launch(const TdxConvInDesc& d, cudaStream_t stream) {
-  ConvInParams p;
-  for (int i = 0; i < 2; ++i) {
-    p.src[i] = d.src[i];
-    p.src_ch[i] = d.src_channels[i];
-    p.src_dtype[i] = d.src_dtype[i];
-    p.src_scale[i] = d.src_scale[i];
-  }
-  p.weight = d.weight;
-  p.ci = d.src_channels[0] + d.src_channels[1] + 1;
-  p.cout = d.c_out;
-  p.H = d.height;
-  p.W = d.width;
-  for (int o = 0; o < 3; ++o) p.out[o] = d.out[o];
-  const int smem = 9 * p.ci * p.cout * 4;
-  int rc_prep = direct_prepare();
-  if (rc_prep != TDX_OK) return rc_prep;
-  dim3 grid((d.height * d.width + 32 * kConvInGroups - 1) / (32 * kConvInGroups), d.n_img);
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, grid, dim3(128), smem, stream);
-  switch (p.ci) {
-    case 6: TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_in_kernel<6>, p)); break;
-    case 12: TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_in_kernel<12>, p)); break;
-    default:
-      set_error("conv_in: %d input channels (incl. ones) not instantiated (6 or 12)", p.ci);
-      return TDX_E_UNSUPPORTED;
-  }
-  return TDX_OK;
-}
 
 // ------------------------------------------------------------------------------------------------ im2col of the input
 struct Im2colParams {
@@ -324,6 +118,8 @@ int im2col_launch(const TdxIm2colDesc& d, cudaStream_t stream) {
 }
 
 // ------------------------------------------------------------------------------------------------ last conv (+ scheduler)
+constexpr int kConvOutGroups = 1;  // conv_out stages only 9*C*COUT weights: more, smaller blocks keep every SM busy
+
 struct ConvOutParams {
   const uint4* x;
   int C8, cout, H, W;
@@ -446,8 +242,6 @@ __global__ void __launch_bounds__(128) conv_out_kernel(const ConvOutParams p) {
 int direct_prepare() {
   static bool seen[16] = {false};
   if (first_use_on_device(seen)) {
-    TDX_CHECK_CUDA(cudaFuncSetAttribute(conv_in_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    TDX_CHECK_CUDA(cudaFuncSetAttribute(conv_in_kernel<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     TDX_CHECK_CUDA(cudaFuncSetAttribute(conv_out_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     TDX_CHECK_CUDA(cudaFuncSetAttribute(conv_out_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   }
@@ -743,13 +537,6 @@ static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t
 }  // namespace tdx
 
 using namespace tdx;
-
-extern "C" int tdx_conv_in_run(const TdxConvInDesc* d, void* stream) {
-  if (!d) { set_error("conv_in: null descriptor"); return TDX_E_INVALID; }
-  int rc = conv_in_validate(*d);
-  if (rc != TDX_OK) return rc;
-  return conv_in_launch(*d, reinterpret_cast<cudaStream_t>(stream));
-}
 
 extern "C" int tdx_im2col_run(const TdxIm2colDesc* d, void* stream) {
   if (!d) { set_error("im2col: null descriptor"); return TDX_E_INVALID; }

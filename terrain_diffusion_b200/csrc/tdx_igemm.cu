@@ -25,8 +25,6 @@
 //   tail of kernel N; griddepcontrol.wait guards everything that depends on earlier kernels.
 //
 // Reference math being replaced: models/mp_layers.py:201-221 (MPConv), models/unet_block.py:116-156 (UNetBlock).
-#include <stdlib.h>
-
 #include "tdx_common.h"
 #include "tdx_ptx.cuh"
 
@@ -38,12 +36,9 @@ constexpr int kKcBytes = kPatchH * kPatchW * 16;  // one 8-channel plane of the 
 constexpr int kAStageBytes = 8 * kKcBytes;        // 64 channels: 23040 B
 constexpr int kSA = 3;                            // A ring depth (max; 2 when the staging tile leaves no room)
 constexpr int kMaxSB = 18;                        // B ring depth (max; also the largest resident weight set)
-#ifndef TDX_EPI_CHUNK
-#define TDX_EPI_CHUNK 32
-#endif
 constexpr int kWQ = 2;                            // epilogue warps per 32-pixel quadrant
 constexpr int kEpiWarps = 4 * kWQ;                // = the two consumer warpgroups
-constexpr int kChunk = TDX_EPI_CHUNK;             // accumulator columns an epilogue warp handles at a time (16 or 32)
+constexpr int kChunk = 32;                        // accumulator columns an epilogue warp handles at a time
 constexpr int kGroups = kChunk / 8;               // 8-channel groups (one uint4 of bf16) per chunk
 constexpr int kThreads = 128 + 32 * kEpiWarps;
 constexpr int kMaxSplit = 8;                      // max CTAs (cluster size) sharing one M tile's pixel-norm statistics
@@ -95,7 +90,6 @@ struct IgemmParams {
   TdxOutSpec out[3];
   float* rms_out;             // optional fp32 [nimg][H][W]: 1 / (eps + rms) of this launch's result
   const float* resid_inv;     // optional fp32 plane at the residual's resolution: r' = r * resid_inv[pixel]
-  int dbg;                    // debug experiment flags (tools/trace_igemm.py), normally 0
   unsigned long long* timeline;  // debug: [2] = {first CTA start, last CTA end} in globaltimer ns, normally null
   unsigned long long* trace;  // debug: per-item phase timestamps of CTA 0 (tools/trace_igemm.py), normally null
 };
@@ -114,33 +108,18 @@ __device__ __forceinline__ void stage_locate(const IgemmParams& p, int s, int& s
   tap = (s - base) - ch * taps;
 }
 
-// Debug hooks (ablation flags, per-item phase clocks, in-graph launch timeline: tools/trace_igemm.py,
-// tools/timeline_forward.py) are compiled in only with -DTDX_DEBUG_HOOKS=1 (TDX_DEBUG_HOOKS=1 python -m
-// terrain_diffusion_b200.build): in the production kernel they would cost ~40 instructions per item and epilogue warp.
+// Debug hooks (per-item phase clocks, in-graph launch timeline: tools/trace_igemm.py, tools/timeline_forward.py) are
+// compiled in only with -DTDX_DEBUG_HOOKS=1 (TDX_DEBUG_HOOKS=1 python -m terrain_diffusion_b200.build): in the
+// production kernel they would cost ~40 instructions per item and epilogue warp.
 #ifndef TDX_DEBUG_HOOKS
 #define TDX_DEBUG_HOOKS 0
 #endif
-// A/B switches (set through TDX_NVCC_DEFINES, see build.py):
-//   TDX_V_TWO_KERNELS  launches without clusters use the cluster-free instantiation (0: one kernel for everything)
-//   TDX_V_AHEAD_R / _C residual / modulation vector fetched one item ahead (R: 0 = at the item's start; C: 0 = in place,
-//                      1 = at the item's start, 2 = one item ahead)
-#ifndef TDX_V_TWO_KERNELS
-#define TDX_V_TWO_KERNELS 1
-#endif
-#ifndef TDX_V_AHEAD_R
-#define TDX_V_AHEAD_R 1
-#endif
-#ifndef TDX_V_AHEAD_C
-#define TDX_V_AHEAD_C 2
-#endif
 #if TDX_DEBUG_HOOKS
-#define TDX_DBG(bit) (p.dbg & (bit))
 #define TDX_TRACE(slot, it)                                                                  \
   do {                                                                                       \
     if (p.trace && blockIdx.x == 0 && (it) < 16) p.trace[(it) * 8 + (slot)] = clock64();     \
   } while (0)
 #else
-#define TDX_DBG(bit) 0
 #define TDX_TRACE(slot, it) do { } while (0)
 #endif
 
@@ -478,13 +457,9 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
         for (int ks = 0; ks < st1 - st0; ++ks) {
           mbar_wait(&b_empty[sb], ph ^ 1);
           if (elect_one()) {
-            if (TDX_DBG(2)) {
-              mbar_arrive(&b_full[sb]);
-            } else {
-              mbar_expect_tx(&b_full[sb], p.b_stage_bytes);
-              bulk_load_1d(bsrc + (size_t)ks * p.b_stage_bytes, &b_full[sb], b_ring + sb * p.b_stage_bytes,
-                           p.b_stage_bytes);
-            }
+            mbar_expect_tx(&b_full[sb], p.b_stage_bytes);
+            bulk_load_1d(bsrc + (size_t)ks * p.b_stage_bytes, &b_full[sb], b_ring + sb * p.b_stage_bytes,
+                         p.b_stage_bytes);
           }
           __syncwarp();
           if (++sb == p.SB) { sb = 0; ph ^= 1; }
@@ -504,13 +479,9 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
           if (first) head = sb;
           if (elect_one()) {
             uint64_t* full = &b_full[head];
-            if (TDX_DBG(2)) {
-              if (first) mbar_arrive(full);
-            } else {
-              if (first) mbar_expect_tx(full, (uint32_t)(nt - t < p.bgroup ? nt - t : p.bgroup) * p.b_stage_bytes);
-              bulk_load_1d(bsrc + (size_t)(ks + t) * p.b_stage_bytes, full, b_ring + sb * p.b_stage_bytes,
-                           p.b_stage_bytes);
-            }
+            if (first) mbar_expect_tx(full, (uint32_t)(nt - t < p.bgroup ? nt - t : p.bgroup) * p.b_stage_bytes);
+            bulk_load_1d(bsrc + (size_t)(ks + t) * p.b_stage_bytes, full, b_ring + sb * p.b_stage_bytes,
+                         p.b_stage_bytes);
           }
           __syncwarp();
           if (++sb == p.SB) { sb = 0; ph ^= 1; }
@@ -597,7 +568,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
       ospec[o] = make_spec(sp, (uint32_t)C8);
       const uint32_t oplane = sp == TDX_SP_DOWN2 ? (plane >> 2) : (sp == TDX_SP_UP2 ? (plane << 2) : plane);
       ospec[o].tpart += (uint32_t)(chbase >> 3) * oplane;
-      if (p.out[o].kind != TDX_OUT_NONE && !(sp == TDX_SP_DOWN2 && ((y | x) & 1)) && !TDX_DBG(16)) omask |= 1u << o;
+      omask |= (uint32_t)(p.out[o].kind != TDX_OUT_NONE && !(sp == TDX_SP_DOWN2 && ((y | x) & 1))) << o;
     }
     // The values an item needs from global memory before it can touch its accumulator are requested ONE ITEM AHEAD
     // (`fetch_ahead`, called where the current item has consumed them): the residual's first-chunk channels or the
@@ -607,8 +578,8 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
     uint4 pre[kPreN];
     const uint4* rbase_pre = nullptr;
     float rinv_pre = 1.f;
-    const bool cv_ahead = (TDX_V_AHEAD_C > 0) && (p.epi & TDX_EPI_EMB_SILU) && !has_resid;   // `pre` holds cvec (else: the residual)
-    const bool ahead = has_resid ? (TDX_V_AHEAD_R != 0) : (cv_ahead && TDX_V_AHEAD_C == 2);   // one item ahead / at the item's start
+    const bool cv_ahead = (p.epi & TDX_EPI_EMB_SILU) && !has_resid;   // `pre` holds cvec (else: the residual)
+    const bool ahead = has_resid || cv_ahead;
     const bool own_rnorm = has_resid && p.resid_pnorm && !p.resid_inv;
     auto fetch_ahead = [&](const TileWalk& t) {
       if (cv_ahead) {
@@ -673,14 +644,13 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
       {
         // ---------------- general: residual mp_sum (+pixel-norm of the residual), clip, pixel-norm, up to 3 outputs
         float rscale = p.resid_scale;
-        if (!ahead) fetch_ahead(tw);
         const uint4* rbase = rbase_pre;
         const bool more = ahead && item + (int)gridDim.x < p.num_items;
         TileWalk tn = tw;
         tn.next(p);
         if (has_resid && p.resid_inv) {
           rscale = p.resid_scale * rinv_pre;
-        } else if (own_rnorm && !TDX_DBG(32)) {
+        } else if (own_rnorm) {
           // the residual's pixel-norm runs over ALL Cout channels: the kWQ warps of a pixel quadrant each read their
           // share of the 8-channel planes (C8 is a multiple of 8) and combine through shared memory
           float ss = 0.f;
@@ -758,7 +728,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
 #pragma unroll
           for (int o = 0; o < 3; ++o) {
             const int kind = p.out[o].kind, sp = p.out[o].spatial;
-            if (kind == TDX_OUT_NONE || (TDX_DBG(64) && o > 0)) continue;
+            if (kind == TDX_OUT_NONE) continue;
             float hs = 0.5f * p.out[o].scale;
             if (kind == TDX_OUT_PNORM_SILU) hs = (p.epi & TDX_EPI_PNORM) ? 0.5f : 0.5f * inv;
             const uint32_t oplane = sp == TDX_SP_DOWN2 ? (plane >> 2) : (sp == TDX_SP_UP2 ? (plane << 2) : plane);
@@ -801,34 +771,32 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
           return inv_rms(tot, p.inv_cout);
         };
 
-        if (!TDX_DBG(4)) {
-          // One code path for all cases (keeps the kernel small enough for the instruction cache): an optional
-          // statistics pass, then the emitting pass.  When every warp has at most one chunk, it stays in registers
-          // across the statistics exchange instead of being recomputed.
-          float v[kChunk];
-          float sumsq = 0.f, inv = 1.f;
-          const bool reuse = need_norm && nchunks <= kWQ;
+        // One code path for all cases (keeps the kernel small enough for the instruction cache): an optional
+        // statistics pass, then the emitting pass.  When every warp has at most one chunk, it stays in registers
+        // across the statistics exchange instead of being recomputed.
+        float v[kChunk];
+        float sumsq = 0.f, inv = 1.f;
+        const bool reuse = need_norm && nchunks <= kWQ;
 #pragma unroll 1
-          for (int pass = need_norm ? 0 : 1; pass < 2; ++pass) {
+        for (int pass = need_norm ? 0 : 1; pass < 2; ++pass) {
 #pragma unroll 1
-            for (int ck = wq; ck < nchunks; ck += kWQ) {
-              if (pass == 0 || !reuse) {
-                compute_v(ck, v);
-                // `pre` (chunk wq of this item) has just been used for the last time: request the next item's
-                if (ck == wq && (reuse || pass == 1) && more) fetch_ahead(tn);
-              }
-              if (pass == 0) {
-#pragma unroll
-                for (int i = 0; i < kChunk; ++i) sumsq = fmaf(v[i], v[i], sumsq);
-              } else {
-                emit_v(ck, v, inv);
-              }
+          for (int ck = wq; ck < nchunks; ck += kWQ) {
+            if (pass == 0 || !reuse) {
+              compute_v(ck, v);
+              // `pre` (chunk wq of this item) has just been used for the last time: request the next item's
+              if (ck == wq && (reuse || pass == 1) && more) fetch_ahead(tn);
             }
             if (pass == 0) {
-              inv = finish_norm(sumsq);
-              if (p.rms_out && wq == 0 && kpart == 0 && tw.split == 0 && valid)
-                p.rms_out[(uint32_t)img * plane + (uint32_t)(Y * p.W + X)] = inv;
+#pragma unroll
+              for (int i = 0; i < kChunk; ++i) sumsq = fmaf(v[i], v[i], sumsq);
+            } else {
+              emit_v(ck, v, inv);
             }
+          }
+          if (pass == 0) {
+            inv = finish_norm(sumsq);
+            if (p.rms_out && wq == 0 && kpart == 0 && tw.split == 0 && valid)
+              p.rms_out[(uint32_t)img * plane + (uint32_t)(Y * p.W + X)] = inv;
           }
         }
       }
@@ -852,7 +820,6 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
 static unsigned long long* g_trace_ptr = nullptr;
 static unsigned long long* g_timeline_ptr = nullptr;   // debug: consecutive launches fill consecutive [start,end] pairs
 static int g_timeline_idx = 0, g_timeline_cap = 0;
-static int g_dbg_flags = 0;
 
 static int ensure_scratch(float** ws);
 
@@ -942,13 +909,10 @@ static int max_active_clusters(int csize) {
 //   * pixel-norm layers exchange statistics inside a cluster, so all nsplit*ks CTAs of an M tile share one (<= 8).
 struct ItemShape { int ncta, resident, sa, sb, ksplit; };
 
-static ItemShape choose_item_shape(int cout, int tiles, int stages, int chunks, int forced_n, bool norm,
-                                   int want_k = 0) {
-  if (!forced_n && getenv("TDX_IGEMM_N")) forced_n = atoi(getenv("TDX_IGEMM_N"));
+static ItemShape choose_item_shape(int cout, int tiles, int stages, int chunks, int forced_n, bool norm) {
   if (forced_n && (forced_n > cout || cout % forced_n)) forced_n = 0;
-  const int forced_k = want_k > 0 ? want_k : (getenv("TDX_IGEMM_KSPLIT") ? atoi(getenv("TDX_IGEMM_KSPLIT")) : 0);
   double best = 1e30;
-  ItemShape bs = {64, 0, kSA, 2, want_k > 0 ? 0 : 1};   // ksplit 0 = "the requested split is not possible"
+  ItemShape bs = {64, 0, kSA, 2, 1};
   for (int n = 64; n <= 256 && n <= cout; n += 64) {
     if (cout % n) continue;
     if (forced_n && n != forced_n) continue;
@@ -965,7 +929,6 @@ static ItemShape choose_item_shape(int cout, int tiles, int stages, int chunks, 
         if (n % (kChunk * ks) || ks > stages || csize > kMaxSplit) continue;
         if (items * ks > (long)max_active_clusters(csize) * csize) continue;   // one item per CTA, all resident
         if ((size_t)items * (ks - 1) * n * 512 > kWsBytes) continue;
-        if (forced_k && ks != forced_k) continue;
       }
       const int my_stages = (stages + ks - 1) / ks;
       const int my_chunks = (chunks + ks - 1) / ks + (ks > 1 ? 1 : 0);
@@ -990,8 +953,6 @@ static ItemShape choose_item_shape(int cout, int tiles, int stages, int chunks, 
       if (l2 > t) t = l2;
       if (per_sm > t) t = per_sm;
       t += epi + red;
-      if (want_k > 0 && ks != want_k) continue;
-      if (forced_k > 1 && ks == 1) t *= 1e6;   // debug override: take the forced split whenever it is valid
       if (t < best) { best = t; bs = {n, resident, sa, sb, ks}; }
     }
   }
@@ -1020,9 +981,7 @@ int igemm_launch(const TdxIgemmDesc& d, const CUtensorMap* tms, cudaStream_t str
   p.tiles_y = (d.height + kTileH - 1) / kTileH;
   const int tiles = p.tiles_x * p.tiles_y * d.n_img;
   const bool norm = needs_norm(d);
-  const ItemShape shp = choose_item_shape(d.c_out, tiles, p.stages_per_item, chunks, d.n_per_item, norm, d.k_split);
-  TDX_REQUIRE(shp.ksplit >= 1, "igemm: k_split=%d is not possible for this launch (n_per_item=%d)", d.k_split,
-              d.n_per_item);
+  const ItemShape shp = choose_item_shape(d.c_out, tiles, p.stages_per_item, chunks, d.n_per_item, norm);
   p.ncta = shp.ncta;
   p.resident = shp.resident;
   p.SA = shp.sa;
@@ -1052,7 +1011,6 @@ int igemm_launch(const TdxIgemmDesc& d, const CUtensorMap* tms, cudaStream_t str
   p.rms_out = d.rms_out;
   p.resid_inv = d.resid_inv;
   p.trace = g_trace_ptr;
-  p.dbg = g_dbg_flags;
   p.timeline = (g_timeline_ptr && g_timeline_idx < g_timeline_cap) ? g_timeline_ptr + 2 * (g_timeline_idx++) : nullptr;
 
   int rc_prep = igemm_prepare();
@@ -1088,7 +1046,7 @@ int igemm_launch(const TdxIgemmDesc& d, const CUtensorMap* tms, cudaStream_t str
     cfg.attrs = attr;
     cfg.numAttrs += 1;
   }
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, igemm_kernel_for(cluster > 1 || !TDX_V_TWO_KERNELS, p.ncta), t0, t1, t2, p));
+  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, igemm_kernel_for(cluster > 1, p.ncta), t0, t1, t2, p));
   return TDX_OK;
 }
 
@@ -1139,7 +1097,6 @@ int igemm_validate(const TdxIgemmDesc& d) {
 extern "C" void tdx_debug_set_igemm_trace(void* device_u64x128) {
   tdx::g_trace_ptr = reinterpret_cast<unsigned long long*>(device_u64x128);
 }
-extern "C" void tdx_debug_set_igemm_flags(int flags) { tdx::g_dbg_flags = flags; }
 // Debug: every igemm launch recorded from now on writes {first CTA start, last CTA end} (globaltimer ns) into the next
 // slot of `device_u64_pairs` (pre-filled with {~0, 0}); pass null to stop.
 extern "C" void tdx_debug_set_igemm_timeline(void* device_u64_pairs, int capacity) {

@@ -19,7 +19,6 @@ sub-sampled or nearest-x2 up-sampled) and the decoder-side activated skip.  Weig
 from __future__ import annotations
 
 import ctypes as C
-import os
 import math
 
 import numpy as np
@@ -27,27 +26,6 @@ import torch
 
 from .. import _lib as L
 from ..layout import pack_weight_segments
-
-
-_TUNED = None
-_TUNED_NEW: dict = {}      # shapes measured in this process (TDX_AUTOTUNE=1); tools/tune_igemm.py writes them out
-_TUNE_CANDIDATES: dict = {}   # TDX_AUTOTUNE=2: valid (N, k_split) per shape key, in program order
-TUNED_PATH = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tuned_shapes.json")
-
-
-def tuned_shapes() -> dict:
-    """{"cout|n|h|w|segments|norm": [n_per_item, k_split]} measured on the GPU (tools/tune_igemm.py)."""
-    global _TUNED
-    if _TUNED is None:
-        _TUNED = {}
-        if os.environ.get("TDX_TUNED_TABLE", "1") != "0":
-            try:
-                import json
-                with open(TUNED_PATH) as f:
-                    _TUNED = dict(json.load(f).get("shapes", {}))
-            except Exception:
-                _TUNED = {}
-    return _TUNED
 
 
 def effective_weight(w: torch.Tensor, gain=1.0) -> torch.Tensor:
@@ -180,8 +158,7 @@ class FoldedWeights:
                 g[f"cond{i}"] = sd[f"conditional_layers.{i}.weight"].contiguous()      # MPEmbedding: un-normalised table
         first = enc[0]
         w_in = effective_weight(sd[f"enc.{first['name']}.weight"])               # [cout][ci][3][3]
-        g["conv_in"] = w_in.permute(2, 3, 1, 0).reshape(9, w_in.shape[1], w_in.shape[0]).contiguous()  # [tap][ci][cout]
-        # the same weights as the [cout][k_pad] matrix of the tensor-core path (tdx_im2col_run + 1x1 igemm):
+        # the first convolution as the [cout][k_pad] matrix of its tensor-core path (tdx_im2col_run + 1x1 igemm):
         # k = tap * ci + c, zero-padded to a multiple of 64
         ci = w_in.shape[1]
         self.conv_in_kpad = ((9 * ci + 63) // 64) * 64
@@ -296,8 +273,6 @@ class UNetEmitter:
             raise ValueError(f"spatial size {h}x{w} must be a multiple of {need} for this model")
         self.fw, self.n, self.h, self.w = fw, n, h, w
         self.dev = fw.device
-        # TDX_CONV_IN_DIRECT=1 selects the CUDA-core first convolution (fp32 inputs / weights) instead of im2col + igemm
-        self.conv_in_direct = os.environ.get("TDX_CONV_IN_DIRECT") == "1"
         self.arena: dict = {}
         self.cvecs: dict = {}
 
@@ -345,7 +320,7 @@ class UNetEmitter:
             res["act"] = self.act(stage_key + ".act", c, hh, ww)
             self._set_out(desc, slot, res["act"], kind, spatial, scale)
             slot += 1
-            if kind == L.OUT_PNORM_SILU and hasattr(desc, "rms_out"):
+            if kind == L.OUT_PNORM_SILU:
                 # the consumer block adds pixelnorm(raw) as its residual: leave it the per-pixel factor (fp32 plane)
                 key = stage_key + ".inv"
                 if key not in self.arena:
@@ -373,7 +348,6 @@ class UNetEmitter:
         d.b_packed = self.fw.packed(wkey, n_item).data_ptr()
         d.c_out = cout
         d.n_img, d.height, d.width = self.n, h, w
-        d._wkey = wkey          # (python-side attribute) lets _add_igemm re-pack for the tuned work-item width
         return d
 
     def _finish_block(self, prog, d, b, key, cout, h, w, nxt, enc_index):
@@ -415,95 +389,9 @@ class UNetEmitter:
         return cur
 
     def _add_igemm(self, prog, d):
-        self._apply_tuned_shape(d)
         L.check(L.lib().tdx_program_add_igemm(prog.handle, C.byref(d)))
         prog.n_igemm += 1
         prog.n_launch += 1
-
-    # ------------------------------------------------------------------ measured (n_per_item, k_split) per launch shape
-    @staticmethod
-    def _shape_key(d) -> str:
-        norm = bool(d.epi_flags & L.EPI_PNORM) or bool(d.rms_out) or any(d.out[o].kind == L.OUT_PNORM_SILU
-                                                                        for o in range(3))
-        segs = ";".join(f"{d.a_channels[i]}x{d.a_taps[i]}" for i in range(d.n_seg))
-        return f"{d.c_out}|{d.n_img}|{d.height}|{d.width}|{segs}|{int(norm)}"
-
-    def _apply_tuned_shape(self, d):
-        """Work-item width N and split-K factor of this launch: from the measured table (tuned_shapes.json, produced on
-        the GPU by tools/tune_igemm.py: the library's cost model is only the fallback), or measured now when
-        TDX_AUTOTUNE=1.  The table is a file, not a run-time search, so every process / rank makes the same choice and
-        multi-GPU results stay bit-identical to single-GPU ones."""
-        wkey = getattr(d, "_wkey", None)
-        if wkey is None:
-            return
-        key = self._shape_key(d)
-        choice = tuned_shapes().get(key)
-        if os.environ.get("TDX_AUTOTUNE") == "2" and key not in _TUNE_CANDIDATES:
-            _TUNE_CANDIDATES[key] = self._valid_shapes(d, wkey)       # tools/tune_igemm.py graph mode
-        if choice is None and os.environ.get("TDX_AUTOTUNE") == "1":
-            choice = self._measure_shape(d, wkey)
-            if choice is not None:
-                tuned_shapes()[key] = choice
-                _TUNED_NEW[key] = choice
-        if choice is None:
-            return
-        n_item, ks = int(choice[0]), int(choice[1])
-        if d.c_out % n_item:
-            return
-        d.n_per_item = n_item
-        d.b_packed = self.fw.packed(wkey, n_item).data_ptr()
-        d.k_split = ks
-
-    def _valid_shapes(self, d, wkey):
-        """Every (N, k_split) this launch accepts (one trial launch each)."""
-        lib = L.lib()
-        out = []
-        keep = (d.n_per_item, d.b_packed, d.k_split)
-        with torch.cuda.device(self.dev):
-            stream = L.current_stream_ptr(self.dev)
-            for n_item in (64, 128, 192, 256):
-                if d.c_out % n_item or n_item > d.c_out:
-                    continue
-                d.n_per_item = n_item
-                d.b_packed = self.fw.packed(wkey, n_item).data_ptr()
-                for ks in (1, 2, 3, 4, 6, 8):
-                    d.k_split = ks
-                    if lib.tdx_igemm_run(C.byref(d), stream) == 0:
-                        out.append([n_item, ks])
-            torch.cuda.synchronize()
-        d.n_per_item, d.b_packed, d.k_split = keep
-        return out
-
-    def _measure_shape(self, d, wkey):
-        """Time every valid (N, k_split) of this launch: median of 5 x 12 back-to-back dependent launches each."""
-        lib = L.lib()
-        best, best_t = None, float("inf")
-        keep = (d.n_per_item, d.b_packed, d.k_split)
-        with torch.cuda.device(self.dev):
-            stream = L.current_stream_ptr(self.dev)
-            for n_item in (64, 128, 192, 256):
-                if d.c_out % n_item or n_item > d.c_out:
-                    continue
-                d.n_per_item = n_item
-                d.b_packed = self.fw.packed(wkey, n_item).data_ptr()
-                for ks in (1, 2, 3, 4, 6, 8):
-                    d.k_split = ks
-                    if lib.tdx_igemm_run(C.byref(d), stream) != 0:
-                        continue
-                    ts = []
-                    for _ in range(5):
-                        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                        e0.record()
-                        for _ in range(12):
-                            lib.tdx_igemm_run(C.byref(d), stream)
-                        e1.record()
-                        torch.cuda.synchronize()
-                        ts.append(e0.elapsed_time(e1))
-                    t = sorted(ts)[len(ts) // 2]
-                    if t < best_t:
-                        best, best_t = (n_item, ks), t
-        d.n_per_item, d.b_packed, d.k_split = keep
-        return list(best) if best else None
 
     # ------------------------------------------------------------------ embedding / modulation vectors
     def emit_embed(self, prog: UNetProgram, labels=None, emb_in=None):
@@ -572,39 +460,26 @@ class UNetEmitter:
             enc_index = idx if side == "enc" else None
             cout = b["cout"]
             if b["kind"] == "conv":
-                cd = L.TdxConvInDesc()
+                # tensor-core first convolution: gather the 3x3 neighbourhoods (tdx_im2col_run), then a 1x1 igemm
+                im = L.TdxIm2colDesc()
                 tot = 0
                 for i, (tensor, ch, scale) in enumerate(srcs):
-                    cd.src[i] = tensor.data_ptr()
-                    cd.src_channels[i] = ch
-                    cd.src_dtype[i] = 0 if tensor.dtype == torch.float32 else 1
-                    cd.src_scale[i] = scale.data_ptr() if scale is not None else None
+                    im.src[i] = tensor.data_ptr()
+                    im.src_channels[i] = ch
+                    im.src_dtype[i] = 0 if tensor.dtype == torch.float32 else 1
+                    im.src_scale[i] = scale.data_ptr() if scale is not None else None
                     tot += ch
                 assert tot + 1 == b["cin"], (tot, b["cin"])
-                if self.conv_in_direct:
-                    # CUDA-core first convolution (fp32 inputs and weights): kept for parity experiments
-                    cd.weight = g["conv_in"].data_ptr()
-                    cd.c_out = cout
-                    cd.n_img, cd.height, cd.width = n, h, w
-                    cur = self._emit_outputs(cd, key, cout, h, w, nxt, enc_index)
-                    L.check(L.lib().tdx_program_add_conv_in(prog.handle, C.byref(cd)))
-                    prog.n_launch += 1
-                else:
-                    # tensor-core first convolution: gather the 3x3 neighbourhoods (tdx_im2col_run), then a 1x1 igemm
-                    im = L.TdxIm2colDesc()
-                    for i in range(2):
-                        im.src[i], im.src_channels[i] = cd.src[i], cd.src_channels[i]
-                        im.src_dtype[i], im.src_scale[i] = cd.src_dtype[i], cd.src_scale[i]
-                    kpad = fw.conv_in_kpad
-                    cols = self.act(key + "im2col", kpad, h, w)
-                    im.out = cols.data_ptr()
-                    im.k_pad = kpad
-                    im.n_img, im.height, im.width = n, h, w
-                    L.check(L.lib().tdx_program_add_im2col(prog.handle, C.byref(im)))
-                    prog.n_launch += 1
-                    d = self._igemm(prog, [(cols, kpad, 1)], "conv_in.im2col", cout, h, w)
-                    cur = self._emit_outputs(d, key, cout, h, w, nxt, enc_index)
-                    self._add_igemm(prog, d)
+                kpad = fw.conv_in_kpad
+                cols = self.act(key + "im2col", kpad, h, w)
+                im.out = cols.data_ptr()
+                im.k_pad = kpad
+                im.n_img, im.height, im.width = n, h, w
+                L.check(L.lib().tdx_program_add_im2col(prog.handle, C.byref(im)))
+                prog.n_launch += 1
+                d = self._igemm(prog, [(cols, kpad, 1)], "conv_in.im2col", cout, h, w)
+                cur = self._emit_outputs(d, key, cout, h, w, nxt, enc_index)
+                self._add_igemm(prog, d)
             elif b["mode"] == "enc":
                 resid_sp = L.SP_SAME
                 if b["resample"] == "down":

@@ -250,16 +250,3 @@ def test_blend_canvas_negative_world_coordinates_and_clipping():
     win = otile.linear_weight_window(16)
     assert torch.equal(cv.wsum.cpu()[:8, :8], win[8:, 8:])
     assert float(cv.wsum.cpu()[8:, :].abs().sum()) == 0.0
-
-
-def test_direct_fp32_first_convolution_variant_matches_reference_golden(monkeypatch):
-    """tdx_conv_in_run (CUDA-core fp32 first convolution, selected at plan time with TDX_CONV_IN_DIRECT=1) is kept as
-    the parity cross-check of the tensor-core im2col path: same forward, same golden."""
-    monkeypatch.setenv("TDX_CONV_IN_DIRECT", "1")
-    cfg = ounet.DECODER_CFG
-    m = EDMUnet2D(**cfg).eval()
-    m.load_state_dict(ounet.procedural_state_dict(cfg, seed=0))
-    m = m.cuda()
-    x, t = _gen_inputs(cfg, 1, 64, seed=1)
-    y = m(x.cuda(), t.cuda(), []).cpu()
-    assert rel_rms(y, torch.from_numpy(G["decoder.y"])) < TOL

@@ -27,7 +27,7 @@ def main():
             best = ms
         else:
             best = [min(a, b) for a, b in zip(best, ms)]
-    names = {0: "conv_in", 1: "igemm", 2: "conv_out", 3: "embed", 4: "attn", 5: "im2col"}
+    names = {1: "igemm", 2: "conv_out", 3: "embed", 4: "attn", 5: "im2col"}
     tot = sum(best)
     print(f"forward {size}x{size} N={n}: sum of per-launch times {tot*1e3:.1f} us over {len(best)} launches")
     agg = {}

@@ -1,8 +1,6 @@
 """Per-tile phase timeline of CTA 0 of the igemm kernel (debug hook tdx_debug_set_igemm_trace).
 
-    python tools/trace_igemm.py [flags]      # flags = OR of the kernel's ablation bits (tdx_debug_set_igemm_flags):
-        2  no weight loads      4  epilogue does nothing      16  compute everything, store nothing
-        32 skip the residual pixel-norm pre-pass      64 only output 0 is produced
+    python tools/trace_igemm.py              # phase clocks of a few launch shapes
     python tools/trace_igemm.py floor        # launch floor of an empty-ish kernel
 """
 import ctypes as C
@@ -31,9 +29,6 @@ def main():
     lib = L.lib()
     lib.tdx_debug_set_igemm_trace.argtypes = [C.c_void_p]
     trace = torch.zeros(128, dtype=torch.int64, device=dev)
-    flags = int(sys.argv[1]) if len(sys.argv) > 1 else 0
-    lib.tdx_debug_set_igemm_flags(flags)
-    print('### debug flags', flags)
     for name, segs, cout, res in SHAPES + [("RES1 64->64 @256 (resid pnorm, 3 outputs)", [(64, 9)], 64, 256)]:
         acts = [to_nc8hw8(torch.randn(1, c, res, res, device=dev)) for c, _ in segs]
         wts = [torch.randn(cout, c, 3, 3, device=dev) * 0.02 for c, t in segs]
@@ -73,7 +68,7 @@ def main():
 
 
 def launch_floor():
-    """Average time per launch of a tiny igemm inside a 200-launch program replayed as a graph (PDL on/off via env)."""
+    """Average time per launch of a tiny igemm inside a 200-launch program replayed as a graph."""
     from terrain_diffusion_b200.models.plan import UNetProgram
     dev = torch.device("cuda:0")
     for name, segs, cout, res in [("tiny 1x1 16x16", [(64, 1)], 64, 16), ("64->64 3x3 @32 (8 items)", [(64, 9)], 64, 32),
@@ -102,7 +97,7 @@ def launch_floor():
             prog.run(True)
         e1.record()
         torch.cuda.synchronize()
-        print(f"launch floor [{name}]: {e0.elapsed_time(e1) / 1000 * 1e3:.2f} us per dependent launch (graph, PDL={os.environ.get('TDX_PDL', '1')})")
+        print(f"launch floor [{name}]: {e0.elapsed_time(e1) / 1000 * 1e3:.2f} us per dependent launch (graph)")
 
 
 if __name__ == "__main__":
