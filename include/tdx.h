@@ -127,6 +127,10 @@ int tdx_im2col_run(const TdxIm2colDesc* desc, void* stream);
  *     F  = conv3x3(x_raw)                          -> model_out (fp32 NCHW, optional)
  *     x0 = c_skip*sample + c_out*F ; sample' = r*sample + (1-r)*x0 + k*(x0 - x0_prev) ; x0_prev = x0
  * coef points at DEVICE floats {c_skip, c_out, r, k}.
+ * Two-model guidance (sample_diffusion_decoder.py:112-117, sample_diffusion_base.py:105-110): with guide_out set, the
+ * guide model's output F_g for this step (fp32 NCHW, written earlier in the stream, e.g. by the guide's own conv_out
+ * with model_out) is combined first, F = F_g + s*(F_m - F_g) (separately rounded: sub, mul, add); coef then points at
+ * five floats {c_skip, c_out, r, k, s} and model_out (if set) receives the combined F.
  * ------------------------------------------------------------------------------------------------------------------ */
 typedef struct TdxConvOutDesc {
   const void* x;           /* bf16 NC8HW8, n_img x c_in x H x W */
@@ -138,6 +142,7 @@ typedef struct TdxConvOutDesc {
   const float* sched_coef; /* DEVICE {c_skip, c_out, r, k} or NULL (no scheduler fusion) */
   float* sample;           /* fp32 NCHW, updated in place (requires sched_coef) */
   float* x0_prev;          /* fp32 NCHW solver history, read+written (requires sched_coef) */
+  const float* guide_out;  /* fp32 NCHW [n_img][c_out][H][W] guide model output, or NULL (requires sched_coef) */
 } TdxConvOutDesc;
 int tdx_conv_out_run(const TdxConvOutDesc* desc, void* stream);
 

@@ -39,7 +39,7 @@ class TdxConvOutDesc(C.Structure):
     _fields_ = [
         ("x", C.c_void_p), ("c_in", C.c_int32), ("weight", C.c_void_p), ("c_out", C.c_int32), ("n_img", C.c_int32),
         ("height", C.c_int32), ("width", C.c_int32), ("model_out", C.c_void_p), ("sched_coef", C.c_void_p),
-        ("sample", C.c_void_p), ("x0_prev", C.c_void_p),
+        ("sample", C.c_void_p), ("x0_prev", C.c_void_p), ("guide_out", C.c_void_p),
     ]
 
 

@@ -128,6 +128,7 @@ struct ConvOutParams {
   const float* coef;
   float* sample;
   float* x0_prev;
+  const float* guide;
 };
 
 // One DPM-Solver++(2M) update in the EDM closed form (scheduler/dpmsolver.py:419-561; SURVEY.md Appendix B).
@@ -140,7 +141,9 @@ __device__ __forceinline__ void sched_update(float x, float f, float x0p, float 
 
 // Block = 128 threads = 32 pixels x 4 sub-threads; sub-thread s accumulates channel groups s, s+4, ... so four times as
 // many 16-byte loads are in flight; the partial sums are combined with two warp shuffles.  COUT = 1 (decoder) or 8.
-template <int COUT>
+// GUIDED: two-model guidance before the update, F = F_g + s*(F_m - F_g) with F_g read from p.guide and s = coef[4]
+// (sample_diffusion_decoder.py:117, sample_diffusion_base.py:110); the unguided instantiations do not contain it.
+template <int COUT, bool GUIDED>
 __global__ void __launch_bounds__(128) conv_out_kernel(const ConvOutParams p) {
   extern __shared__ float ws[];  // [tap][c][COUT]
   const int C = p.C8 * 8;
@@ -223,10 +226,16 @@ __global__ void __launch_bounds__(128) conv_out_kernel(const ConvOutParams p) {
     if (!inb || sub != 0) continue;
     float cs = 0.f, co = 0.f, r = 0.f, k = 0.f;
     if (p.coef) { cs = __ldg(p.coef); co = __ldg(p.coef + 1); r = __ldg(p.coef + 2); k = __ldg(p.coef + 3); }
+    float gs = 0.f;
+    if constexpr (GUIDED) gs = __ldg(p.coef + 4);
 #pragma unroll
     for (int oc = 0; oc < COUT; ++oc) {
       if (oc >= p.cout) break;
       const size_t idx = ((size_t)img * p.cout + oc) * plane + pix;
+      if constexpr (GUIDED) {
+        const float fg = p.guide[idx];   // written by the guide model's conv_out launch earlier in the stream
+        acc[oc] = __fadd_rn(fg, __fmul_rn(gs, __fsub_rn(acc[oc], fg)));
+      }
       if (p.model_out) p.model_out[idx] = acc[oc];
       if (p.coef) {
         float xn, x0;
@@ -242,8 +251,14 @@ __global__ void __launch_bounds__(128) conv_out_kernel(const ConvOutParams p) {
 int direct_prepare() {
   static bool seen[16] = {false};
   if (first_use_on_device(seen)) {
-    TDX_CHECK_CUDA(cudaFuncSetAttribute(conv_out_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    TDX_CHECK_CUDA(cudaFuncSetAttribute(conv_out_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    TDX_CHECK_CUDA(cudaFuncSetAttribute(conv_out_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        200 * 1024));
+    TDX_CHECK_CUDA(cudaFuncSetAttribute(conv_out_kernel<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        200 * 1024));
+    TDX_CHECK_CUDA(cudaFuncSetAttribute(conv_out_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        200 * 1024));
+    TDX_CHECK_CUDA(cudaFuncSetAttribute(conv_out_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        200 * 1024));
   }
   return TDX_OK;
 }
@@ -255,6 +270,7 @@ int conv_out_validate(const TdxConvOutDesc& d) {
   TDX_REQUIRE(9 * d.c_in * 8 * 4 <= 200 * 1024, "conv_out: c_in=%d too large", d.c_in);
   TDX_REQUIRE(d.model_out || d.sched_coef, "conv_out: nothing to write");
   if (d.sched_coef) TDX_REQUIRE(d.sample && d.x0_prev, "conv_out: scheduler fusion needs sample and x0_prev");
+  TDX_REQUIRE(!d.guide_out || d.sched_coef, "conv_out: guide_out needs sched_coef (the guidance scale is coef[4])");
   return TDX_OK;
 }
 
@@ -270,6 +286,7 @@ int conv_out_launch(const TdxConvOutDesc& d, cudaStream_t stream) {
   p.coef = d.sched_coef;
   p.sample = d.sample;
   p.x0_prev = d.x0_prev;
+  p.guide = d.guide_out;
   const int wout = d.c_out == 1 ? 1 : 8;
   const int smem = 9 * d.c_in * wout * 4;
   int rc_prep = direct_prepare();
@@ -278,8 +295,13 @@ int conv_out_launch(const TdxConvOutDesc& d, cudaStream_t stream) {
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[1];
   fill_launch_config(&cfg, attr, grid, dim3(128), smem, stream);
-  if (wout == 1) TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_out_kernel<1>, p));
-  else TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_out_kernel<8>, p));
+  if (d.guide_out) {
+    if (wout == 1) TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_out_kernel<1, true>, p));
+    else TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_out_kernel<8, true>, p));
+  } else {
+    if (wout == 1) TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_out_kernel<1, false>, p));
+    else TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_out_kernel<8, false>, p));
+  }
   return TDX_OK;
 }
 

@@ -45,20 +45,29 @@ def _solve_cache(model):
     return model._solve_cache
 
 
-def get_diffusion_solve(model, scheduler, n, h, w, num_steps, step_range=None) -> DiffusionSolve:
+def get_diffusion_solve(model, scheduler, n, h, w, num_steps, step_range=None, guide=None, guidance_scale: float = 1.0,
+                        score_scaling: float = 1.0) -> DiffusionSolve:
     """Cached fused N-step solve (or one phase of it: step_range).  The key is everything the solve bakes in: the
     sigma table and the per-step order schedule (they cover sigma_min/max/rho/schedule, scaling_p/scaling_t,
-    lower_order_final, euler_at_final, ...) plus the options that change the update formula.  The caller's scheduler
-    is put in the state the reference leaves it in (`set_timesteps(num_steps)`) on a cache hit too."""
+    lower_order_final, euler_at_final, ...) plus the options that change the update formula, and for a guided solve
+    the guide's weights, the guidance scale and the score scaling.  The caller's scheduler is put in the state the
+    reference leaves it in (`set_timesteps(num_steps)`) on a cache hit too."""
     scheduler.set_timesteps(num_steps)
     c = scheduler.config
     key = (n, h, w, num_steps, None if step_range is None else tuple(int(v) for v in step_range),
            tuple(float(v) for v in scheduler.sigmas), tuple(scheduler.order_schedule()),
            float(c.sigma_data), c.prediction_type, c.final_sigmas_type, c.solver_order, c.algorithm_type, c.solver_type,
            id(model.folded()))
+    guided = guide is not None and float(guidance_scale) != 1.0
+    if guided:
+        key += ("guide", id(guide.folded()), float(guidance_scale))
+    if score_scaling != 1.0:
+        key += ("score_scaling", float(score_scaling))
     cache = _solve_cache(model)
     if key not in cache:
-        cache[key] = DiffusionSolve(model, scheduler, n, h, w, num_steps, step_range=step_range)
+        cache[key] = DiffusionSolve(model, scheduler, n, h, w, num_steps, step_range=step_range,
+                                    guide=guide if guided else None, guidance_scale=guidance_scale,
+                                    score_scaling=score_scaling)
     return cache[key]
 
 
@@ -79,10 +88,9 @@ def sample_decoder_diffusion_tiled(model, scheduler, cond_img: torch.Tensor, noi
                                    tile_size: Optional[int] = None, tile_stride: Optional[int] = None, *,
                                    num_steps: Optional[int] = None, guidance_model=None, guidance_scale: float = 1.0,
                                    score_scaling: float = 1.0, weight_window_fn=None, tile_batch: int = 1):
-    if guidance_model is not None and guidance_scale != 1.0:
-        raise NotImplementedError("two-model guidance is not on the product path and is not implemented")
-    if score_scaling != 1.0:
-        raise NotImplementedError("score_scaling != 1 is not on the product path and is not implemented")
+    """guidance_model / guidance_scale: two-model guidance F = F_g + s*(F_m - F_g) inside the fused solve (both
+    forwards and the combination in one graph; the guide must have multiples of 64 channels in every layer).
+    score_scaling: the reference's EDM score scaling (`_scale_score`), folded into the step coefficients."""
     if num_steps is None:
         num_steps = scheduler.num_inference_steps
         if num_steps is None:
@@ -103,7 +111,8 @@ def sample_decoder_diffusion_tiled(model, scheduler, cond_img: torch.Tensor, noi
     for g0 in range(0, len(tiles), group):
         chunk = tiles[g0:g0 + group]
         n = b * len(chunk)
-        solve = get_diffusion_solve(model, scheduler, n, tile_size, tile_size, num_steps)
+        solve = get_diffusion_solve(model, scheduler, n, tile_size, tile_size, num_steps, guide=guidance_model,
+                                    guidance_scale=guidance_scale, score_scaling=score_scaling)
         x = torch.cat([noise32[..., i0:i0 + tile_size, j0:j0 + tile_size] for (i0, j0) in chunk], dim=0)
         cd = torch.cat([cond32[..., i0:i0 + tile_size, j0:j0 + tile_size] for (i0, j0) in chunk], dim=0)
         out = solve.run(x, cd)
@@ -111,6 +120,81 @@ def sample_decoder_diffusion_tiled(model, scheduler, cond_img: torch.Tensor, noi
             for bi in range(b):
                 canvases[bi].accumulate(out[t * b + bi], i0, j0, window)
     return torch.stack([cv.normalized() for cv in canvases]).to(dtype)
+
+
+def _reference_cond_vector(tile_cond, histogram_raw, cond_means, cond_stds, noise_level):
+    """sample_diffusion_base.py:11-48 (`_process_cond_img`) for one window: the NaN handling of the reference's
+    evaluation sampler (batch ROWS 0 and 1, unseeded randn for NaN climate means) on top of the product's vector."""
+    from .stages import process_latent_conditioning
+    return process_latent_conditioning(tile_cond, histogram_raw, cond_means, cond_stds, noise_level,
+                                       reference_sampler_nans=True)
+
+
+@torch.no_grad()
+def sample_base_diffusion(model, scheduler, shape, cond_inputs, *, cond_means, cond_stds, noise_level=0.0,
+                          histogram_raw, dtype=torch.float32, steps: int = 15, guide_model=None,
+                          guidance_scale: float = 1.0, generator: Optional[torch.Generator] = None,
+                          tile_size: Optional[int] = None, weight_window_fn=None, tile_batch: Optional[int] = None):
+    """The base model's diffusion sampler (training/evaluation/sample_diffusion_base.py:51-168), optionally with
+    two-model guidance; every N-step solve is one fused graph (both models per step when guided).
+
+    Untiled (tile_size None): `cond_inputs` is passed to the model as given (a list of conditional inputs) and the
+    result is NOT divided by sigma_data.  Tiled: stride tile_size // 2; each tile's 58-dim condition vector comes from
+    the [ic:ic+4, jc:jc+4] window of the (len(starts)+3)-sized cond image; each tile starts from a fresh solver; tiles
+    are blended in row-major order and the result is divided by sigma_data.  Independent tiles are solved
+    `tile_batch` at a time (default: all at once); the blend order, and so the result, does not depend on it.
+
+    The initial noise is torch.randn(shape, generator=generator) * sigma_0 as the reference draws it; a CPU generator
+    draws on the CPU and the noise is copied to the model's device."""
+    from .tiling import linear_weight_window as _lww
+    device = model.device
+    scheduler.set_timesteps(steps)
+    sigma0 = float(scheduler.sigmas[0])      # sigma_max: the same for every step count
+    gen_dev = generator.device if generator is not None else device
+    noise = torch.randn(tuple(shape), generator=generator, device=gen_dev, dtype=dtype)
+    noise = (noise * torch.tensor(sigma0, dtype=torch.float32).to(noise.device)).to(device)
+    B, C, H, W = shape
+    if tile_size is None:
+        solve = get_diffusion_solve(model, scheduler, B, H, W, steps, guide=guide_model, guidance_scale=guidance_scale)
+        out = solve.run(noise.float(), None, conditional_inputs=[torch.as_tensor(c).to(device) for c in cond_inputs])
+        return out.clone().to(dtype)
+
+    stride = tile_size // 2
+    h_starts, w_starts = tile_starts(H, tile_size, stride), tile_starts(W, tile_size, stride)
+    cond_inputs = torch.as_tensor(cond_inputs)
+    if cond_inputs.ndim == 1 and len(h_starts) * len(w_starts) > 1:
+        raise ValueError(f"cond_inputs must be a tensor image for tiled sampling. Cond inputs must have width "
+                         f"{len(w_starts)+3} and height {len(h_starts)+3}.")
+    elif cond_inputs.ndim == 4:
+        if cond_inputs.shape[-1] != len(w_starts) + 3 or cond_inputs.shape[-2] != len(h_starts) + 3:
+            raise ValueError(f"cond_inputs is {tuple(cond_inputs.shape[-2:])}; tiled sampling of {H}x{W} needs "
+                             f"{len(h_starts)+3}x{len(w_starts)+3}")
+    window = (weight_window_fn(tile_size, device, torch.float32)[0, 0] if weight_window_fn is not None
+              else _lww(tile_size, device)).contiguous()
+    tiles = [(ic, i0, jc, j0) for ic, i0 in enumerate(h_starts) for jc, j0 in enumerate(w_starts)]
+    # every tile's condition vector, in tile order (the reference computes them in this order too: the unseeded NaN
+    # fill draws from the global generator one tile after the other)
+    if cond_inputs.ndim == 4:
+        cimg = cond_inputs.to(device)
+        cvecs = [_reference_cond_vector(cimg[..., ic:ic + 4, jc:jc + 4], histogram_raw, cond_means, cond_stds,
+                                        noise_level) for ic, _, jc, _ in tiles]
+    else:
+        cvecs = [cond_inputs.to(device).float().reshape(1, -1).expand(B, -1)] * len(tiles)
+    canvas = [BlendCanvas(C, H, W, device) for _ in range(B)]
+    group = len(tiles) if tile_batch is None else max(1, int(tile_batch))
+    for g0 in range(0, len(tiles), group):
+        chunk = list(range(g0, min(g0 + group, len(tiles))))
+        solve = get_diffusion_solve(model, scheduler, B * len(chunk), tile_size, tile_size, steps, guide=guide_model,
+                                    guidance_scale=guidance_scale)
+        x = torch.cat([noise[..., tiles[t][1]:tiles[t][1] + tile_size, tiles[t][3]:tiles[t][3] + tile_size]
+                       for t in chunk], dim=0).float()
+        cv = torch.cat([cvecs[t] for t in chunk], dim=0)
+        out = solve.run(x, None, conditional_inputs=[cv])
+        for k, t in enumerate(chunk):
+            for bi in range(B):
+                canvas[bi].accumulate(out[k * B + bi], tiles[t][1], tiles[t][3], window)
+    sd = float(scheduler.config.sigma_data)
+    return torch.stack([cv.normalized(sd) for cv in canvas]).to(dtype)
 
 
 @torch.no_grad()

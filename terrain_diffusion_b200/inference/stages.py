@@ -116,20 +116,34 @@ def _concat_scales(dims, dev) -> torch.Tensor:
 
 
 @torch.no_grad()
-def process_latent_conditioning(cond_img, histogram_raw, cond_means, cond_stds, noise_level, seed=0, seed_offset=0):
+def process_latent_conditioning(cond_img, histogram_raw, cond_means, cond_stds, noise_level, seed=0, seed_offset=0,
+                                reference_sampler_nans: bool = False):
     """The 58-dim condition vector of the base model for a batch of coarse windows (world_pipeline.py:1018-1050):
     cond_img [n, 7, 4, 4] = de-blended coarse channels + mask.  Batched, on cond_img's device, no host round trip.
     The reference replaces every NaN of its batch-of-one tensor by cond_means[0] before it looks for NaNs in the climate
     crop, so its seeded NaN fill (:1040-1044) can never trigger; `seed` / `seed_offset` are accepted for signature
-    compatibility."""
+    compatibility.  histogram_raw is [H] (shared) or [n, H] (per row); noise_level a scalar, [1] or [n, 1].
+    reference_sampler_nans: the NaN handling of the evaluation sampler's `_process_cond_img`
+    (sample_diffusion_base.py:36-46) instead: NaNs of batch ROW 0 become cond_means[0], of row 1 cond_means[1], and
+    NaN climate means are filled with unseeded standard normals (SURVEY Appendix G)."""
     dev = cond_img.device
     n = cond_img.shape[0]
     cond_means = torch.as_tensor(cond_means)
     x = (cond_img.float() - _const_on(dev, cond_means).view(1, -1, 1, 1)) / _const_on(dev, cond_stds).view(1, -1, 1, 1)
-    x = torch.nan_to_num(x, nan=float(cond_means.flatten()[0]))
+    if reference_sampler_nans:
+        cm = cond_means.flatten()
+        x[0:1] = torch.nan_to_num(x[0:1], nan=float(cm[0]))
+        x[1:2] = torch.nan_to_num(x[1:2], nan=float(cm[1]))
+    else:
+        x = torch.nan_to_num(x, nan=float(cond_means.flatten()[0]))
     level = _const_on(dev, ((torch.as_tensor(noise_level, dtype=torch.float32).cpu() - 0.5) * math.sqrt(12)).reshape(-1, 1))
-    hist = _const_on(dev, histogram_raw).reshape(1, -1)
-    parts = [x[:, 0].flatten(1), x[:, 1].flatten(1), x[:, 2:6, 1:3, 1:3].mean(dim=(2, 3)), x[:, 6].flatten(1),
+    hist = _const_on(dev, histogram_raw)
+    hist = hist.reshape(1, -1) if hist.dim() < 2 else hist
+    clim = x[:, 2:6, 1:3, 1:3].mean(dim=(2, 3))
+    if reference_sampler_nans:
+        bad = torch.isnan(clim)
+        clim[bad] = torch.randn_like(clim[bad])
+    parts = [x[:, 0].flatten(1), x[:, 1].flatten(1), clim, x[:, 6].flatten(1),
              hist.expand(n, -1), level.expand(n, -1)]
     return torch.cat(parts, dim=1) * _concat_scales([p.shape[1] for p in parts], dev)
 

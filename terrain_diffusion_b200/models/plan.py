@@ -444,7 +444,8 @@ class UNetEmitter:
 
     def _emit(self, prog: UNetProgram, srcs, model_out=None, sched=None, cvec_set: int = 0):
         """srcs: [(tensor NCHW fp32/bf16, channels, scale_ptr_tensor or None)] (1 or 2 sources);
-        model_out: fp32 [n, Cout, h, w] or None; sched: None or dict(coef=tensor[4], sample=tensor, x0_prev=tensor);
+        model_out: fp32 [n, Cout, h, w] or None; sched: None or dict(coef=tensor[4], sample=tensor, x0_prev=tensor)
+        [+ guide_out=fp32 tensor like sample, with coef=tensor[5] ending in the guidance scale];
         cvec_set: which label set's modulation vectors (see emit_embed) this evaluation uses."""
         fw = self.fw
         g = fw.g
@@ -557,6 +558,8 @@ class UNetEmitter:
             od.sched_coef = sched["coef"].data_ptr()
             od.sample = sched["sample"].data_ptr()
             od.x0_prev = sched["x0_prev"].data_ptr()
+            if sched.get("guide_out") is not None:
+                od.guide_out = sched["guide_out"].data_ptr()     # two-model guidance: coef holds 5 floats
         L.check(L.lib().tdx_program_add_conv_out(prog.handle, C.byref(od)))
         prog.n_launch += 1
         prog.keep.append((self.arena, self.cvecs, fw, srcs, model_out, sched))
