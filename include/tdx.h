@@ -68,7 +68,7 @@ typedef struct TdxIgemmDesc {
   int32_t n_seg;
   /* B operand: packed bf16 weights [c_out/n_per_item slices][stage = (segment, 64-ch chunk, tap)][8][n_per_item][8] */
   const void* b_packed;
-  int32_t c_out;           /* multiple of 64, <= 256 */
+  int32_t c_out;           /* multiple of 64, <= 2048 */
   int32_t n_per_item;      /* output channels per work item = MMA N the weights were packed for (tdx_igemm_choose_n) */
   int32_t n_img, height, width;   /* output == input spatial size; multiples of 8 */
   /* epilogue */
@@ -163,8 +163,8 @@ typedef struct TdxEmbedDesc {
   const float* emb_in;         /* DEVICE fp32 [n_img][emb_channels] precomputed embedding, or NULL */
   const float* noise_weight;   /* fp32 effective, TRANSPOSED [noise_dims][emb_channels] */
   const float* noise_freqs;    /* DEVICE fp32 [noise_dims/2]: the model's MPPositionalEmbedding.freqs buffer */
-  int32_t noise_dims;          /* even, <= 256 */
-  int32_t emb_channels;        /* <= 1024 */
+  int32_t noise_dims;          /* multiple of 4, <= 256 */
+  int32_t emb_channels;        /* multiple of 16, <= 1024 */
   int32_t n_img;
   int32_t n_blocks;
   const TdxEmbedBlock* blocks; /* HOST array of n_blocks entries (copied by the call) */

@@ -93,6 +93,9 @@ def _declare(l: C.CDLL) -> None:
                                      C.POINTER(C.c_int32), C.c_int32]
     l.tdx_igemm_run.restype = C.c_int
     l.tdx_igemm_run.argtypes = [C.POINTER(TdxIgemmDesc), C.c_void_p]
+    l.tdx_debug_igemm_plan.restype = None
+    l.tdx_debug_igemm_plan.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32),
+                                       C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32)]
     l.tdx_abi_sizeof.restype = C.c_int
     l.tdx_abi_sizeof.argtypes = [C.c_int]
     for i, st in enumerate(ABI_STRUCTS):

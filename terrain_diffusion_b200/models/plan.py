@@ -18,6 +18,7 @@ sub-sampled or nearest-x2 up-sampled) and the decoder-side activated skip.  Weig
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import math
 
@@ -237,6 +238,13 @@ class UNetProgram:
         self.n_igemm = 0
         self.n_launch = 0
 
+    def add(self, kind: str, desc):
+        """Append one launch: kind = igemm | im2col | attn | embed | conv_out, desc = the matching Tdx*Desc."""
+        L.check(getattr(L.lib(), f"tdx_program_add_{kind}")(self.handle, C.byref(desc)))
+        self.n_launch += 1
+        if kind == "igemm":
+            self.n_igemm += 1
+
     def run(self, use_graph: bool = True):
         L.call(L.lib().tdx_program_run, self.device, self.handle, 1 if use_graph else 0)
 
@@ -276,14 +284,24 @@ class UNetEmitter:
         self.arena: dict = {}
         self.cvecs: dict = {}
 
+    def _buffer(self, shape, dtype, fill=None):
+        """Every device buffer the emitter owns (activations, pixel-norm planes, modulation vectors) comes from here."""
+        if fill is None:
+            return torch.empty(shape, dtype=dtype, device=self.dev)
+        return torch.full(shape, fill, dtype=dtype, device=self.dev)
+
+    def _device_scope(self):
+        # planning allocates per-device library scratch and asks per-device questions: the model's device is current
+        return torch.cuda.device(self.dev) if self.dev.type == "cuda" else contextlib.nullcontext()
+
     def act(self, key, c, h, w):
         if key not in self.arena:
-            self.arena[key] = torch.empty((self.n, c // 8, h, w, 8), dtype=torch.bfloat16, device=self.dev)
+            self.arena[key] = self._buffer((self.n, c // 8, h, w, 8), torch.bfloat16)
         return self.arena[key]
 
     def cvec(self, key, c):
         if key not in self.cvecs:
-            self.cvecs[key] = torch.ones((self.cvec_sets * self.n, c), dtype=torch.float32, device=self.dev)
+            self.cvecs[key] = self._buffer((self.cvec_sets * self.n, c), torch.float32, fill=1.0)
         return self.cvecs[key]
 
     # ------------------------------------------------------------------ helpers
@@ -324,7 +342,7 @@ class UNetEmitter:
                 # the consumer block adds pixelnorm(raw) as its residual: leave it the per-pixel factor (fp32 plane)
                 key = stage_key + ".inv"
                 if key not in self.arena:
-                    self.arena[key] = torch.empty((self.n, h, w), dtype=torch.float32, device=self.dev)
+                    self.arena[key] = self._buffer((self.n, h, w), torch.float32)
                 res["inv"] = self.arena[key]
                 desc.rms_out = res["inv"].data_ptr()
         if enc_index is not None and enc_index in self.fw.skip_consumer:
@@ -357,26 +375,25 @@ class UNetEmitter:
         if not b["heads"]:
             d.clip = fw.clip
             cur = self._emit_outputs(d, key, cout, h, w, nxt, enc_index)
-            self._add_igemm(prog, d)
+            prog.add("igemm", d)
             return cur
         # ---- attention: x1 = mp_sum(x, y) un-clipped -> q, k, v (1x1) -> softmax core -> proj (1x1) + mp_sum + clip
         x1 = self.act(key + "x1", cout, h, w)
         d.clip = 0.0
         self._set_out(d, 0, x1, L.OUT_RAW)
-        self._add_igemm(prog, d)
+        prog.add("igemm", d)
         qkv = []
         for nm in ("q", "k", "v"):
             t = self.act(key + nm, cout, h, w)
             dq = self._igemm(prog, [(x1, cout, 1)], key + nm, cout, h, w)
             self._set_out(dq, 0, t, L.OUT_RAW)
-            self._add_igemm(prog, dq)
+            prog.add("igemm", dq)
             qkv.append(t)
         yat = self.act(key + "attn_y", cout, h, w)
         ad = L.TdxAttnDesc()
         ad.q, ad.k, ad.v, ad.out = qkv[0].data_ptr(), qkv[1].data_ptr(), qkv[2].data_ptr(), yat.data_ptr()
         ad.n_img, ad.heads, ad.head_dim, ad.tokens = self.n, b["heads"], fw.cph, h * w
-        L.check(L.lib().tdx_program_add_attn(prog.handle, C.byref(ad)))
-        prog.n_launch += 1
+        prog.add("attn", ad)
         dp = self._igemm(prog, [(yat, cout, 1)], key + "proj", cout, h, w)
         ta = fw.t_attn
         dp.epi_flags = L.EPI_RESID
@@ -385,18 +402,12 @@ class UNetEmitter:
         dp.resid_scale = (1 - ta) / math.sqrt((1 - ta) ** 2 + ta ** 2)
         dp.clip = fw.clip
         cur = self._emit_outputs(dp, key, cout, h, w, nxt, enc_index)
-        self._add_igemm(prog, dp)
+        prog.add("igemm", dp)
         return cur
-
-    def _add_igemm(self, prog, d):
-        L.check(L.lib().tdx_program_add_igemm(prog.handle, C.byref(d)))
-        prog.n_igemm += 1
-        prog.n_launch += 1
 
     # ------------------------------------------------------------------ embedding / modulation vectors
     def emit_embed(self, prog: UNetProgram, labels=None, emb_in=None):
-        # (planning allocates per-device library scratch and asks per-device questions: the model's device is current)
-        with torch.cuda.device(self.dev):
+        with self._device_scope():
             return self._emit_embed(prog, labels, emb_in)
 
     def _emit_embed(self, prog: UNetProgram, labels=None, emb_in=None):
@@ -430,8 +441,7 @@ class UNetEmitter:
         ed.n_img = rows
         ed.n_blocks = len(blocks)
         ed.blocks = arr
-        L.check(L.lib().tdx_program_add_embed(prog.handle, C.byref(ed)))
-        prog.n_launch += 1
+        prog.add("embed", ed)
         prog.keep.append((labels, emb_in))
 
     def _cvec_ptr(self, key, c, cvec_set):
@@ -439,7 +449,7 @@ class UNetEmitter:
 
     # ------------------------------------------------------------------ one U-Net evaluation
     def emit(self, prog: UNetProgram, srcs, model_out=None, sched=None, cvec_set: int = 0):
-        with torch.cuda.device(self.dev):
+        with self._device_scope():
             return self._emit(prog, srcs, model_out, sched, cvec_set)
 
     def _emit(self, prog: UNetProgram, srcs, model_out=None, sched=None, cvec_set: int = 0):
@@ -476,11 +486,10 @@ class UNetEmitter:
                 im.out = cols.data_ptr()
                 im.k_pad = kpad
                 im.n_img, im.height, im.width = n, h, w
-                L.check(L.lib().tdx_program_add_im2col(prog.handle, C.byref(im)))
-                prog.n_launch += 1
+                prog.add("im2col", im)
                 d = self._igemm(prog, [(cols, kpad, 1)], "conv_in.im2col", cout, h, w)
                 cur = self._emit_outputs(d, key, cout, h, w, nxt, enc_index)
-                self._add_igemm(prog, d)
+                prog.add("igemm", d)
             elif b["mode"] == "enc":
                 resid_sp = L.SP_SAME
                 if b["resample"] == "down":
@@ -493,7 +502,7 @@ class UNetEmitter:
                     a_in = self.act(key + "a0", cout, h, w)
                     self._set_out(d, 0, xn, L.OUT_RAW)
                     self._set_out(d, 1, a_in, L.OUT_SILU, L.SP_SAME, 1.0)
-                    self._add_igemm(prog, d)
+                    prog.add("igemm", d)
                     resid, resid_pn, resid_inv = xn, 0, None
                 else:
                     a_in, resid, resid_pn = cur["act"], cur["raw"], 1
@@ -505,7 +514,7 @@ class UNetEmitter:
                 d.epi_flags = L.EPI_EMB_SILU
                 d.cvec = self._cvec_ptr(key, cout, cvec_set)
                 self._set_out(d, 0, hbuf, L.OUT_RAW)
-                self._add_igemm(prog, d)
+                prog.add("igemm", d)
                 d = self._igemm(prog, [(hbuf, cout, 9)], key + "res1", cout, h, w)
                 d.epi_flags = L.EPI_RESID
                 d.resid = resid.data_ptr()
@@ -532,7 +541,7 @@ class UNetEmitter:
                 d.epi_flags = L.EPI_EMB_SILU
                 d.cvec = self._cvec_ptr(key, cout, cvec_set)
                 self._set_out(d, 0, hbuf, L.OUT_RAW)
-                self._add_igemm(prog, d)
+                prog.add("igemm", d)
                 if b.get("concat"):
                     d = self._igemm(prog, [(hbuf, cout, 9), (cur["raw"], cx, 1), (sk["raw"], cs, 1)], key + "res1",
                                     cout, h, w)
@@ -560,7 +569,6 @@ class UNetEmitter:
             od.x0_prev = sched["x0_prev"].data_ptr()
             if sched.get("guide_out") is not None:
                 od.guide_out = sched["guide_out"].data_ptr()     # two-model guidance: coef holds 5 floats
-        L.check(L.lib().tdx_program_add_conv_out(prog.handle, C.byref(od)))
-        prog.n_launch += 1
+        prog.add("conv_out", od)
         prog.keep.append((self.arena, self.cvecs, fw, srcs, model_out, sched))
         prog.arena = self.arena

@@ -1,7 +1,7 @@
-"""Plain-PyTorch fp32 reference of ONE tdx_igemm_run launch (conv + fused epilogue), and a runner for the CUDA op.
+"""Plain-PyTorch fp64 reference of ONE tdx_igemm_run launch (conv + fused epilogue), and a runner for the CUDA op.
 
-Used by tests/test_igemm_gpu.py and tools/bringup_igemm.py.  Inputs are rounded to bf16 first so that the only
-difference to the kernel is accumulation order and the bf16 rounding of the stored outputs.
+Used by tests/test_igemm_gpu.py, tests/test_igemm_plans_gpu.py and tools/bringup_igemm.py.  Inputs are rounded to bf16
+first so that the only difference to the kernel is accumulation order and the bf16 rounding of the stored outputs.
 """
 from __future__ import annotations
 
@@ -13,6 +13,10 @@ import torch.nn.functional as F
 
 from terrain_diffusion_b200 import _lib as L
 from terrain_diffusion_b200.layout import from_nc8hw8, pack_weight_segments, to_nc8hw8
+
+TILE_H, TILE_W = 16, 8          # pixels of one work item (kTileH x kTileW in tdx_igemm.cu)
+GUARD_BYTES = 4096              # sentinel before and after every output buffer
+SENTINEL16, SENTINEL32 = 0x5A5B, 0x5A5B5C5D
 
 
 def mp_silu(x):
@@ -40,48 +44,119 @@ class Case:
     wscale: float = 1.0
     n_item: int = 0   # 0 = let the library choose (tdx_igemm_choose_n)
     seed: int = 0
+    rms_out: bool = False     # the launch also stores 1 / (eps + rms) of its result per pixel
+    resid_inv: bool = False   # the residual's pixel-norm comes from a precomputed plane (needs resid_pnorm)
+
+    @property
+    def macs(self) -> int:
+        return self.n * self.h * self.w * self.cout * sum(c * t for c, t in self.segs)
+
+
+def case_from_desc(d, name: str = "desc", seed: int = 0) -> Case:
+    """The Case that replays descriptor `d` (a TdxIgemmDesc recorded from the product) with fresh inputs: same segments,
+    shape, work-item width, epilogue, residual mode, pixel-norm side planes, scale, clip and outputs."""
+    segs = [(int(d.a_channels[i]), int(d.a_taps[i])) for i in range(d.n_seg)]
+    outs = [(int(o.kind), int(o.spatial), float(o.scale)) for o in d.out if o.kind != L.OUT_NONE]
+    resid_inv = bool(d.resid_inv)
+    return Case(name, segs, int(d.c_out), int(d.n_img), int(d.height), int(d.width), epi=int(d.epi_flags),
+                resid_spatial=int(d.resid_spatial), resid_pnorm=1 if resid_inv else int(d.resid_pnorm),
+                resid_scale=float(d.resid_scale), clip=float(d.clip), outs=outs, n_item=int(d.n_per_item), seed=seed,
+                rms_out=bool(d.rms_out), resid_inv=resid_inv)
+
+
+def needs_norm(case: Case) -> bool:
+    """Whether the launch computes per-pixel statistics over all c_out channels (as igemm_launch decides it)."""
+    return bool(case.epi & L.EPI_PNORM) or case.rms_out or any(k == L.OUT_PNORM_SILU for k, _, _ in case.outs)
+
+
+def device_sm_count() -> int:
+    sm, ma, mi = C.c_int(), C.c_int(), C.c_int()
+    L.check(L.lib().tdx_device_info(C.byref(sm), C.byref(ma), C.byref(mi)))
+    return sm.value
+
+
+def plan_of(case: Case, sm_count: int | None = None) -> dict:
+    """The launch plan igemm_launch makes for this case on the current device: work-item width N, split-K factor,
+    resident weights or ring depth SB, cluster size, and the grid it derives from them (rounds = work items per CTA,
+    `partial` = the last round leaves some CTAs idle).  `ragged` = the height is not a multiple of the 16-row tile."""
+    ch = (C.c_int32 * 3)(*[c for c, _ in case.segs], *([0] * (3 - len(case.segs))))
+    tp = (C.c_int32 * 3)(*[t for _, t in case.segs], *([0] * (3 - len(case.segs))))
+    n_item = case.n_item or L.igemm_choose_n(case.cout, case.n, case.h, case.w, case.segs)
+    norm = needs_norm(case)
+    out = (C.c_int32 * 4)()
+    L.lib().tdx_debug_igemm_plan(case.cout, case.n, case.h, case.w, ch, tp, len(case.segs), n_item, int(norm), out)
+    N, ks, resident, sb = (int(v) for v in out)
+    nsplit = case.cout // N
+    cluster = nsplit * ks if (norm and nsplit * ks > 1) else ks
+    tiles = -(-case.h // TILE_H) * -(-case.w // TILE_W) * case.n
+    items = tiles * nsplit * ks
+    sms = device_sm_count() if sm_count is None else sm_count
+    grid = min(items, sms)
+    grid -= grid % (nsplit * ks)
+    rounds = -(-items // grid)
+    return dict(N=N, ks=ks, resident=resident, SB=sb, cluster=cluster, nsplit=nsplit, items=items, grid=grid,
+                rounds=rounds, partial=items % grid != 0, ragged=case.h % TILE_H != 0)
+
+
+def plan_class(p: dict) -> tuple:
+    """(N, ksplit, resident, SB, cluster size, more than one round, ragged): what makes two launches take different
+    paths through the kernel."""
+    return (p["N"], p["ks"], p["resident"], p["SB"], p["cluster"], p["rounds"] > 1, p["ragged"])
+
+
+def plan_label(cls: tuple) -> str:
+    N, ks, res, sb, cl, multi, ragged = cls
+    return (f"N{N}-ks{ks}-{'res' if res else 'SB'}{sb}-cl{cl}-{'multi' if multi else 'one'}"
+            f"{'-ragged' if ragged else ''}")
 
 
 def make_inputs(case: Case, device):
-    g = torch.Generator(device="cpu").manual_seed(case.seed)
+    """bf16-exact activations, weights and residual, fp32 modulation vector (drawn on `device`: a 40-image case takes
+    milliseconds)."""
+    device = torch.device(device)
+    g = torch.Generator(device=device).manual_seed(case.seed)
     acts, wts = [], []
     ktot = sum(c * t for c, t in case.segs)
     for (c, t) in case.segs:
-        a = torch.randn(case.n, c, case.h, case.w, generator=g)
+        a = torch.randn(case.n, c, case.h, case.w, generator=g, device=device)
         k = 3 if t == 9 else 1
-        w = torch.randn(case.cout, c, k, k, generator=g) * (case.wscale / ktot ** 0.5)
-        acts.append(a.bfloat16().float().to(device))
-        wts.append(w.bfloat16().float().to(device))
-    cvec = (1.0 + 0.3 * torch.randn(case.n, case.cout, generator=g)).to(device)
-    if case.resid_spatial == L.SP_UP2:
-        rs = (case.h // 2, case.w // 2)
-    elif case.resid_spatial == L.SP_DOWN2:
-        rs = (case.h * 2, case.w * 2)
-    else:
-        rs = (case.h, case.w)
-    resid = torch.randn(case.n, case.cout, *rs, generator=g).bfloat16().float().to(device)
+        w = torch.randn(case.cout, c, k, k, generator=g, device=device) * (case.wscale / ktot ** 0.5)
+        acts.append(a.bfloat16().float())
+        wts.append(w.bfloat16().float())
+    cvec = 1.0 + 0.3 * torch.randn(case.n, case.cout, generator=g, device=device)
+    resid = torch.randn(case.n, case.cout, *resid_size(case), generator=g, device=device).bfloat16().float()
     return acts, wts, cvec, resid
 
 
+def resid_size(case: Case) -> tuple:
+    if case.resid_spatial == L.SP_UP2:
+        return (case.h // 2, case.w // 2)
+    if case.resid_spatial == L.SP_DOWN2:
+        return (case.h * 2, case.w * 2)
+    return (case.h, case.w)
+
+
 def reference(case: Case, acts, wts, cvec, resid):
+    """fp64 outputs of the launch; with case.rms_out one more entry: the fp64 plane 1 / (eps + rms) of the result."""
     acc = None
     for a, w in zip(acts, wts):
         y = F.conv2d(a.double(), w.double(), padding=w.shape[-1] // 2)
         acc = y if acc is None else acc + y
-    v = acc.float()
+    v = acc
     if case.epi & L.EPI_EMB_SILU:
-        v = mp_silu(v * cvec[:, :, None, None])
+        v = mp_silu(v * cvec.double()[:, :, None, None])
     if case.epi & L.EPI_RESID:
-        r = resid
+        r = resid.double()
+        if case.resid_pnorm:
+            r = pixelnorm(r)
         if case.resid_spatial == L.SP_UP2:
             r = r.repeat_interleave(2, dim=2).repeat_interleave(2, dim=3)
         elif case.resid_spatial == L.SP_DOWN2:
             r = r[:, :, ::2, ::2]
-        if case.resid_pnorm:
-            r = pixelnorm(r)
         v = v + case.resid_scale * r
     if case.clip > 0:
         v = torch.clamp(v, -case.clip, case.clip)
+    inv = 1.0 / (1e-4 + v.square().mean(dim=1).sqrt())
     if case.epi & L.EPI_PNORM:
         v = pixelnorm(v)
     outs = []
@@ -97,10 +172,44 @@ def reference(case: Case, acts, wts, cvec, resid):
         elif spatial == L.SP_UP2:
             o = o.repeat_interleave(2, dim=2).repeat_interleave(2, dim=3)
         outs.append(o)
+    if case.rms_out:
+        outs.append(inv)
     return outs
 
 
+class Guarded:
+    """A tensor view inside a larger allocation with GUARD_BYTES of sentinel on each side: check() fails if the kernel
+    wrote outside the view.  The view starts 16-byte aligned and is NaN-filled, so an unwritten element fails too."""
+
+    def __init__(self, shape, dtype, device):
+        self.dtype = dtype
+        raw = torch.int16 if dtype == torch.bfloat16 else torch.int32
+        self.sentinel = SENTINEL16 if dtype == torch.bfloat16 else SENTINEL32
+        esz = torch.empty((), dtype=dtype).element_size()
+        self.pad = GUARD_BYTES // esz
+        numel = 1
+        for s in shape:
+            numel *= s
+        self.numel = numel
+        self.raw = torch.full((self.pad + numel + self.pad,), self.sentinel, dtype=raw, device=device)
+        self.view = self.raw[self.pad:self.pad + numel].view(dtype).view(*shape)
+        self.view.fill_(float("nan"))
+        assert self.view.data_ptr() % 16 == 0
+
+    def data_ptr(self):
+        return self.view.data_ptr()
+
+    def check(self, what):
+        before, after = self.raw[:self.pad], self.raw[self.pad + self.numel:]
+        bad = int((before != self.sentinel).sum()) + int((after != self.sentinel).sum())
+        assert bad == 0, f"{what}: {bad} elements written outside the tensor"
+
+
 def run_cuda(case: Case, acts, wts, cvec, resid, rms_out=None, resid_inv=None):
+    """One tdx_igemm_run launch.  Every bf16 output (and, with case.rms_out, the fp32 rms plane, returned last) lives
+    in a guarded buffer whose sentinels are checked after the launch.  case.resid_inv: the residual's pixel-norm plane
+    is computed here from `resid` and passed as resid_inv.  The rms_out / resid_inv arguments pass caller-owned planes
+    instead."""
     dev = acts[0].device
     a_dev = [to_nc8hw8(a) for a in acts]
     n_item = case.n_item or L.igemm_choose_n(case.cout, case.n, case.h, case.w, case.segs)
@@ -121,7 +230,13 @@ def run_cuda(case: Case, acts, wts, cvec, resid, rms_out=None, resid_inv=None):
     d.cvec = cvec_dev.data_ptr()
     d.resid = r_dev.data_ptr()
     d.resid_spatial = case.resid_spatial
+    if resid_inv is None and case.resid_inv:
+        resid_inv = (1.0 / (1e-4 + resid.double().square().mean(dim=1).sqrt())).float().contiguous()
     d.resid_pnorm = case.resid_pnorm if resid_inv is None else 0
+    rms_guard = None
+    if rms_out is None and case.rms_out:
+        rms_guard = Guarded((case.n, case.h, case.w), torch.float32, dev)
+        rms_out = rms_guard.view
     if rms_out is not None:        # fp32 [n, h, w]: 1 / (eps + rms) of the result, for the consumer's residual
         d.rms_out = rms_out.data_ptr()
     if resid_inv is not None:      # fp32 plane at the residual's resolution: replaces the recomputed pixel-norm
@@ -135,7 +250,7 @@ def run_cuda(case: Case, acts, wts, cvec, resid, rms_out=None, resid_inv=None):
             hh, ww = hh // 2, ww // 2
         elif spatial == L.SP_UP2:
             hh, ww = hh * 2, ww * 2
-        o = torch.full((case.n, case.cout // 8, hh, ww, 8), float("nan"), dtype=torch.bfloat16, device=dev)
+        o = Guarded((case.n, case.cout // 8, hh, ww, 8), torch.bfloat16, dev)
         bufs.append(o)
         d.out[i].ptr = o.data_ptr()
         d.out[i].kind = kind
@@ -143,11 +258,62 @@ def run_cuda(case: Case, acts, wts, cvec, resid, rms_out=None, resid_inv=None):
         d.out[i].scale = scale
     L.check(L.lib().tdx_igemm_run(C.byref(d), L.current_stream_ptr()))
     torch.cuda.synchronize()
-    return [from_nc8hw8(o) for o in bufs]
+    for i, o in enumerate(bufs):
+        o.check(f"{case.name} out{i}")
+    res = [from_nc8hw8(o.view) for o in bufs]
+    if rms_guard is not None:
+        rms_guard.check(f"{case.name} rms_out")
+        res.append(rms_guard.view.clone())
+    return res
+
+
+def report(config, lines):
+    """Write `lines` to the terminal past pytest's output capture, so summaries show under `pytest -q` too."""
+    tr = config.pluginmanager.get_plugin("terminalreporter")
+    capman = config.pluginmanager.get_plugin("capturemanager")
+    if tr is None or capman is None:
+        print("\n".join(lines))
+        return
+    with capman.global_and_fixture_disabled():
+        tr.write("\n")                      # off the line of progress dots
+        for line in lines:
+            tr.write_line(line)
 
 
 def rel_rms(a, b):
     return float((a - b).square().mean().sqrt() / (b.square().mean().sqrt() + 1e-30))
+
+
+def elementwise_ratio(got, ref) -> float:
+    """max over elements of |got - ref| / (2^-7 |ref| + 2^-12 rms(ref)), ref in fp64: one bf16 ulp (twice the worst
+    rounding error, room for a rounding flip after fp32 accumulation) plus a floor for cancellation in the residual
+    sum.  <= 1 passes; NaN anywhere in `got` fails."""
+    ref = ref.double()
+    err = (got.double() - ref).abs()
+    bound = 2.0 ** -7 * ref.abs() + 2.0 ** -12 * float(ref.square().mean().sqrt())
+    if torch.isnan(err).any():
+        return float("inf")
+    return float((err / bound).max())
+
+
+def check_case(case: Case, device, margins: dict | None = None):
+    """Run `case` on the GPU against the fp64 reference: rel-RMS < 2e-3 against the bf16-rounded reference and the
+    per-element bound of elementwise_ratio on every output (and the rms plane).  Returns the worst ratio."""
+    acts, wts, cvec, resid = make_inputs(case, device)
+    refs = reference(case, acts, wts, cvec, resid)
+    gots = run_cuda(case, acts, wts, cvec, resid)
+    worst = 0.0
+    for i, (g, r) in enumerate(zip(gots, refs)):
+        what = f"{case.name} {'rms_out' if i == len(case.outs) else f'out{i}'}"
+        assert not torch.isnan(g).any(), f"{what}: unwritten (NaN) elements"
+        if i < len(case.outs):
+            assert rel_rms(g, r.bfloat16().double()) < 2e-3, what
+        ratio = elementwise_ratio(g, r)
+        worst = max(worst, ratio)
+        assert ratio <= 1.0, f"{what}: error {ratio:.2f}x the per-element bound"
+    if margins is not None:
+        margins[case.name] = worst
+    return worst
 
 
 def default_cases() -> list[Case]:

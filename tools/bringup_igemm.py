@@ -14,7 +14,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 
 from terrain_diffusion_b200 import _lib as L
-from tests._igemm_ref import Case, default_cases, make_inputs, reference, rel_rms, run_cuda
+from tests._igemm_ref import default_cases, make_inputs, plan_of, reference, rel_rms, run_cuda
 
 LOG = []
 
@@ -90,13 +90,9 @@ def main():
     for case in default_cases():
         try:
             acts, wts, cvec, resid = make_inputs(case, dev)
-            plan = (C.c_int32 * 4)()
-            ch = (C.c_int32 * 3)(*[c for c, _ in case.segs], *([0] * (3 - len(case.segs))))
-            tp = (C.c_int32 * 3)(*[t for _, t in case.segs], *([0] * (3 - len(case.segs))))
-            n_item = case.n_item or L.igemm_choose_n(case.cout, case.n, case.h, case.w, case.segs)
-            norm = int(bool(case.epi & L.EPI_PNORM) or any(k == L.OUT_PNORM_SILU for k, _, _ in case.outs))
-            L.lib().tdx_debug_igemm_plan(case.cout, case.n, case.h, case.w, ch, tp, len(case.segs), n_item, norm, plan)
-            log(f"     plan {case.name}: N={plan[0]} ksplit={plan[1]} resident={plan[2]} SB={plan[3]}")
+            plan = plan_of(case)
+            log(f"     plan {case.name}: N={plan['N']} ksplit={plan['ks']} resident={plan['resident']} SB={plan['SB']} "
+                f"cluster={plan['cluster']} rounds={plan['rounds']}")
             refs = reference(case, acts, wts, cvec, resid)
             gots = run_cuda(case, acts, wts, cvec, resid)
             worst = 0.0
