@@ -1,7 +1,8 @@
 """Mirror of the sampling part of terrain_diffusion.inference / terrain_diffusion.training.evaluation."""
 from .canvas import BlendCanvas  # noqa: F401
-from .samplers import (sample_base_diffusion, sample_decoder_consistency_tiled,  # noqa: F401
-                       sample_decoder_diffusion_sharded, sample_decoder_diffusion_tiled)
+from .samplers import (sample_base_consistency, sample_base_diffusion, sample_coarse_tiled,  # noqa: F401
+                       sample_decoder_consistency_tiled, sample_decoder_diffusion_sharded,
+                       sample_decoder_diffusion_tiled)
 from .sharded import ShardedCanvas  # noqa: F401
 from .solve import DiffusionSolve, fold_score_scaling  # noqa: F401
 from .tiling import linear_weight_window, padded_batch_size, shard_rows, tile_starts, window_range  # noqa: F401

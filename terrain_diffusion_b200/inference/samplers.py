@@ -1,6 +1,6 @@
 """Bounded-canvas tiled samplers -- drop-ins for terrain_diffusion.training.evaluation.sample_diffusion_decoder
-(reference sample_diffusion_decoder.py:44-211), running tile solves as fused CUDA graphs and the overlap blend on a
-device-resident canvas.
+(reference sample_diffusion_decoder.py:44-211), .sample_diffusion_base and .sample_coarse, running tile solves as
+fused CUDA graphs and the overlap blend on a device-resident canvas.
 
 Tile order, tile origins (`tile_starts`, last tile clamped) and the blend window are the reference's, integer for
 integer.  Unlike the reference function as shipped, the multi-tile diffusion sampler resets the solver state per tile
@@ -195,6 +195,164 @@ def sample_base_diffusion(model, scheduler, shape, cond_inputs, *, cond_means, c
                 canvas[bi].accumulate(out[k * B + bi], tiles[t][1], tiles[t][3], window)
     sd = float(scheduler.config.sigma_data)
     return torch.stack([cv.normalized(sd) for cv in canvas]).to(dtype)
+
+
+def _phase_times(scheduler, intermediate_t, dtype) -> list:
+    """Consistency times as the reference's evaluation sampler forms them (sample_diffusion_base.py:216-220): the fp32
+    atan(sigma_0 / sigma_d) cast to `dtype`, then intermediate_t if > 0; returned as the floats of those tensors."""
+    sigma_data = float(scheduler.config.sigma_data)
+    ts = [float(torch.atan(scheduler.sigmas[0] / sigma_data).to(dtype))]
+    if intermediate_t > 0:
+        ts.append(float(torch.tensor(intermediate_t, dtype=dtype)))
+    return ts
+
+
+@torch.no_grad()
+def sample_base_consistency(model, scheduler, shape, cond_inputs, *, cond_means, cond_stds, noise_level=0.0,
+                            histogram_raw, intermediate_t=0.0, dtype=torch.float32,
+                            generator: Optional[torch.Generator] = None, tile_size: Optional[int] = None,
+                            weight_window_fn=None, noise=None, tile_batch: Optional[int] = None):
+    """The base consistency model's evaluation sampler (training/evaluation/sample_diffusion_base.py:171-268): one
+    TrigFlow step per phase at t_0 = atan(sigma_0 / sigma_d), then at `intermediate_t` if > 0.
+
+    Per phase: x_t = cos t * s + sin t * sigma_d * z per tile (s = 0 in the first phase, the previous phase's blended
+    canvas after it), s' = cos t * x_t - sin t * sigma_d * pred with pred = -model(x_t / sigma_d, t, [cvec]), tiles of
+    stride tile_size // 2 blended in row-major order and normalised; the result is divided by sigma_d.  Every phase
+    of `tile_batch` tiles (default: all) is one fused consistency program (get_consistency_solve); the blend order,
+    and so the canvas, does not depend on the grouping, the implicit-GEMM work split does (DESIGN section 2).
+
+    z is noise[k] if given, else one torch.randn(shape, generator=generator) per phase, drawn on the generator's device
+    before that phase's tiles and copied to the model's device.  A 4-D `cond_inputs` is the (len(starts)+3)-sized
+    condition image: each tile's vector comes from its [ic:ic+4, jc:jc+4] window, recomputed every phase as the
+    reference does (its unseeded NaN-climate fill draws in (phase, tile) order); any other tensor is the condition
+    vector itself, for every tile."""
+    if tile_size is None:
+        raise ValueError("sample_base_consistency samples in tiles: tile_size is required")
+    B, C, H, W = shape
+    stride = tile_size // 2
+    h_starts, w_starts = tile_starts(H, tile_size, stride), tile_starts(W, tile_size, stride)
+    cond_inputs = torch.as_tensor(cond_inputs)
+    if cond_inputs.ndim == 1 and len(h_starts) * len(w_starts) > 1:
+        raise ValueError(f"cond_inputs must be a tensor image for tiled sampling. Cond inputs must have width "
+                         f"{len(w_starts)+3} and height {len(h_starts)+3}.")
+    elif cond_inputs.ndim == 4:
+        if cond_inputs.shape[-1] != len(w_starts) + 3 or cond_inputs.shape[-2] != len(h_starts) + 3:
+            raise ValueError(f"cond_inputs is {tuple(cond_inputs.shape[-2:])}; tiled sampling of {H}x{W} needs "
+                             f"{len(h_starts)+3}x{len(w_starts)+3}")
+    if noise is not None and len(noise) < 1 + (intermediate_t > 0):
+        raise ValueError(f"noise has {len(noise)} phases; this call runs {1 + (intermediate_t > 0)}")
+    from .stages import trig_mix
+    device = model.device
+    sigma_data = float(scheduler.config.sigma_data)
+    ts = _phase_times(scheduler, intermediate_t, dtype)
+    T = tile_size
+    window = (weight_window_fn(T, device, torch.float32)[0, 0] if weight_window_fn is not None
+              else linear_weight_window(T, device)).contiguous()
+    tiles = [(ic, i0, jc, j0) for ic, i0 in enumerate(h_starts) for jc, j0 in enumerate(w_starts)]
+    group = len(tiles) if tile_batch is None else max(1, int(tile_batch))
+    gen_dev = generator.device if generator is not None else device
+    if cond_inputs.ndim == 4:
+        cimg = cond_inputs.to(device)
+    else:
+        cv = cond_inputs.to(device).float()
+        cv = cv.reshape(1, -1) if cv.ndim == 1 else cv
+        fixed = cv.expand(B, *cv.shape[1:])
+    sample = None                                           # the previous phase's normalised canvas [B, C, H, W]
+    for k, t in enumerate(ts):
+        z = (torch.randn(tuple(shape), generator=generator, device=gen_dev, dtype=dtype) if noise is None
+             else torch.as_tensor(noise[k]))
+        z = z.to(device).float()
+        if cond_inputs.ndim == 4:
+            cvecs = [_reference_cond_vector(cimg[..., ic:ic + 4, jc:jc + 4], histogram_raw, cond_means, cond_stds,
+                                            noise_level) for ic, _, jc, _ in tiles]
+        else:
+            cvecs = [fixed] * len(tiles)
+        canvas = [BlendCanvas(C, H, W, device) for _ in range(B)]
+        for g0 in range(0, len(tiles), group):
+            chunk = tiles[g0:g0 + group]
+            zt = torch.cat([z[..., i0:i0 + T, j0:j0 + T] for _, i0, _, j0 in chunk], dim=0).contiguous()
+            if sample is None:
+                x = zt                                      # s = 0: x_t = sin t sigma_d z, folded into the program
+            else:
+                st = torch.cat([sample[..., i0:i0 + T, j0:j0 + T] for _, i0, _, j0 in chunk], dim=0).contiguous()
+                x = trig_mix(st, zt, math.cos(t), math.sin(t) * sigma_data)
+            solve = get_consistency_solve(model, B * len(chunk), T, T, t, sigma_data, from_unit_noise=sample is None)
+            out = solve.run(x, None, conditional_inputs=[torch.cat(cvecs[g0:g0 + len(chunk)], dim=0)])
+            for q, (_, i0, _, j0) in enumerate(chunk):
+                for bi in range(B):
+                    canvas[bi].accumulate(out[q * B + bi], i0, j0, window)
+        last = k == len(ts) - 1
+        sample = torch.stack([cv.normalized(sigma_data if last else 1.0) for cv in canvas])
+    return sample.to(dtype)
+
+
+def cond_inputs_from_snr(cond_snr, device, dtype) -> list:
+    """The coarse model's float conditions from the per-channel SNR of its conditioning image
+    (training/evaluation/sample_coarse.py:7-26): log(tan(atan(snr)) / 8) in `dtype`, one [rows] tensor per channel."""
+    snr = torch.as_tensor(cond_snr).to(device=device, dtype=dtype)
+    vals = torch.log(torch.tan(torch.atan(snr)) / 8.0)
+    return [vals[:, i].contiguous() for i in range(vals.shape[1])]
+
+
+@torch.no_grad()
+def sample_coarse_tiled(model, scheduler, cond_img: torch.Tensor, cond_snr, *, steps: int = 15,
+                        tile_size: Optional[int] = None, tile_stride: Optional[int] = None, weight_window_fn=None,
+                        generator: Optional[torch.Generator] = None, dtype=torch.float32,
+                        tile_batch: Optional[int] = None):
+    """The coarse model's sampler (training/evaluation/sample_coarse.py:29-125): a `steps`-step DPM-Solver++ solve per
+    tile, conditioned on the noised conditioning image and on the five float conditions of `cond_snr`.
+
+    cond_snr is [1, C_cond]: one SNR per conditioning channel, shared by the batch.  (The reference runs this shape
+    at batch 1 only; with more images its [1]-row conditions fail to stack against the [B]-row noise embedding.)
+    The conditioning image is noised first, as cos t_c * cond_img + sin t_c * torch.randn_like(cond_img) with
+    t_c = atan(cond_snr), from the global generator of cond_img's device; then every tile draws
+    torch.randn(tile, generator=generator) * sigma_0 on cond_img's device, in row-major tile order.  tile_size
+    defaults to the image width, tile_stride to tile_size.  Each tile's solve is one fused graph; `tile_batch` tiles
+    (default: all) are solved together.  Each tile is divided by sigma_d, blended in row-major order and normalised;
+    the result is [B, out_channels, H, W] on cond_img's device, in `dtype`.
+
+    Unlike the reference function as shipped, every tile starts from a reset solver: the reference raises IndexError
+    on the second tile because its stateful scheduler is never reset (SURVEY.md section 0 item 7), so its only
+    working case, one tile, is reproduced and the multi-tile result is the per-tile-reset one."""
+    if cond_img.ndim != 4:
+        raise ValueError(f"cond_img must be [B, C, H, W]; got shape {tuple(cond_img.shape)}")
+    b, c_cond, h, w = cond_img.shape
+    cond_snr = torch.as_tensor(cond_snr)
+    if cond_snr.ndim != 2 or cond_snr.shape[0] != 1 or cond_snr.shape[1] != c_cond:
+        raise ValueError(f"cond_snr must be [1, {c_cond}] (one SNR per conditioning channel, shared by the batch); "
+                         f"got shape {tuple(cond_snr.shape)}")
+    tile_size = tile_size or w
+    tile_stride = tile_stride or tile_size
+    if tile_size > h or tile_size > w:
+        raise ValueError(f"tile_size {tile_size} is larger than the {h}x{w} image")
+    device, src = model.device, cond_img.device
+    out_channels = int(model.config.get("out_channels") or model.config["in_channels"])
+    T = tile_size
+    window = (weight_window_fn(T, device, torch.float32)[0, 0] if weight_window_fn is not None
+              else linear_weight_window(T, device)).contiguous()
+    cond_inputs = [ci.to(device) for ci in cond_inputs_from_snr(cond_snr, src, dtype)]
+    t_cond = torch.atan(cond_snr).view(1, -1, 1, 1).to(src)
+    cond_img = torch.cos(t_cond) * cond_img + torch.sin(t_cond) * torch.randn_like(cond_img)
+    scheduler.set_timesteps(int(steps))
+    sigma0 = scheduler.sigmas[0].to(src)
+    tiles = [(i0, j0) for i0 in tile_starts(h, T, tile_stride) for j0 in tile_starts(w, T, tile_stride)]
+    noise = [(torch.randn((b, out_channels, T, T), device=src, generator=generator) * sigma0).to(device)
+             for _ in tiles]
+    cond_d = cond_img.to(device).float()
+    sd = float(scheduler.config.sigma_data)
+    canvas = [BlendCanvas(out_channels, h, w, device) for _ in range(b)]
+    group = len(tiles) if tile_batch is None else max(1, int(tile_batch))
+    for g0 in range(0, len(tiles), group):
+        chunk = tiles[g0:g0 + group]
+        n = b * len(chunk)
+        solve = get_diffusion_solve(model, scheduler, n, T, T, int(steps))
+        x = torch.cat(noise[g0:g0 + len(chunk)], dim=0).float()
+        cd = torch.cat([cond_d[..., i0:i0 + T, j0:j0 + T] for (i0, j0) in chunk], dim=0)
+        out = solve.run(x, cd, conditional_inputs=[ci.float().expand(n).contiguous() for ci in cond_inputs]) / sd
+        for q, (i0, j0) in enumerate(chunk):
+            for bi in range(b):
+                canvas[bi].accumulate(out[q * b + bi], i0, j0, window)
+    return torch.stack([cv.normalized() for cv in canvas]).to(device=src, dtype=dtype)
 
 
 @torch.no_grad()
