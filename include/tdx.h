@@ -261,6 +261,36 @@ int tdx_climate_sample(const float* t_sea, const float* beta, const float* coars
                        int32_t crop, const float* elev, int32_t i1, int32_t j1, int32_t h, int32_t w,
                        int32_t coarse_stride, int32_t ci1, int32_t cj1, float* out, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Shaded relief map (get_relief_map, inference/relief_map.py:64-199), which the reference renders on the CPU from a
+ * copied elevation window.  terrain_diffusion_b200/inference/relief.py composes the three calls: stats, then (after the
+ * host picks the NaN fill from stats[0]) both Gaussian filters, then the fused shade-and-colour kernel.  Elevation and
+ * planes are contiguous fp32 [h][w].
+ * ------------------------------------------------------------------------------------------------------------------ */
+/* One pass over elev[n] (relief_map.py:107,135-140): stats[0] = NaN count, stats[1] = ~bits(nanmin(max(0, elev))),
+ * stats[2] = bits(nanmax(max(0, elev))).  stats is a DEVICE uint32[3]; the call zeroes it first. */
+int tdx_relief_stats(const float* elev, int64_t n, uint32_t* stats, void* stream);
+/* scipy.ndimage.gaussian_filter(x, sigma_s) for n_sigma (1 or 2) filters at once (relief_map.py:125-126): mode
+ * 'reflect' (half-sample symmetric, any radius), axis 0 then axis 1, accumulated in double as scipy's symmetric
+ * correlate1d does (x[i]*w[0], then + (x[i-k] + x[i+k])*w[k] for k = r..1) and rounded to fp32 after each axis.
+ * weights: HOST fp64, the 2*radius[s]+1 normalised taps of each filter back to back (must be symmetric);
+ * radius[s] <= 96.  replace_nan != 0 reads NaN input as nan_fill (the reference's np.nan_to_num, :107-109).
+ * tmp and out: n_sigma x h x w fp32 each; out[s] is the result of filter s. */
+int tdx_relief_gaussian(const float* x, int32_t h, int32_t w, int32_t replace_nan, float nan_fill, int32_t n_sigma,
+                        const double* weights, const int32_t* radius, float* tmp, float* out, void* stream);
+/* RGB [h][w][3] fp32 (relief_map.py:111-199 without biome, rgb or river inputs): np.gradient + hillshade of
+ * blurred[0] (sigma_large) and blurred[1] (sigma_small) with dy, dx divided by grad_div = 15*resolution/90, sun at
+ * az_rad and sin_alt / cos_alt of the 45 degree altitude; 0.75/0.25 mix, ^0.85; colour from lut (DEVICE [256][3],
+ * matplotlib `terrain` cast to fp32) at norm = (max(0, elev) - vmin) / denom; intensity * relief + one_minus_relief;
+ * NaN where elev is NaN; ocean blend where the NaN-filled elevation is below 0.  With user_range == 0 the colour range
+ * comes from `stats` (tdx_relief_stats on this elev; non-finite or empty range -> [0, 1]) and vmin, denom and
+ * vmin_is_zero are ignored; otherwise vmin = fp32(max(0, vmin)), denom = fp32(vmax - vmin + 1e-8) and vmin_is_zero
+ * selects the 0.25 + 0.75 * clip(norm^0.7) branch.  h, w >= 2. */
+int tdx_relief_shade(const float* elev, const float* blurred, const uint32_t* stats, const float* lut, int32_t h,
+                     int32_t w, int32_t replace_nan, float nan_fill, float grad_div, double az_rad, double sin_alt,
+                     double cos_alt, float relief, float one_minus_relief, int32_t user_range, float vmin, float denom,
+                     int32_t vmin_is_zero, float* out, void* stream);
+
 /* Tile-seeded N(0,1) field, bit-exact with inference/portable_rng.py + world_pipeline.py:66-115 */
 int tdx_noise_patch(uint64_t base_seed, int64_t y0, int64_t x0, int32_t h, int32_t w, int32_t channels,
                     int32_t tile_h, int32_t tile_w, float* out, void* workspace, int64_t workspace_bytes,

@@ -145,6 +145,15 @@ def _declare(l: C.CDLL) -> None:
     l.tdx_climate_sample.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                      C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                      C.c_int32, C.c_void_p, C.c_void_p]
+    l.tdx_relief_stats.restype = C.c_int
+    l.tdx_relief_stats.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    l.tdx_relief_gaussian.restype = C.c_int
+    l.tdx_relief_gaussian.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_int32,
+                                      C.POINTER(C.c_double), C.POINTER(C.c_int32), C.c_void_p, C.c_void_p, C.c_void_p]
+    l.tdx_relief_shade.restype = C.c_int
+    l.tdx_relief_shade.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                   C.c_float, C.c_float, C.c_double, C.c_double, C.c_double, C.c_float, C.c_float,
+                                   C.c_int32, C.c_float, C.c_float, C.c_int32, C.c_void_p, C.c_void_p]
     l.tdx_noise_patch.restype = C.c_int
     l.tdx_noise_patch.argtypes = [C.c_uint64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                   C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]

@@ -9,5 +9,6 @@ from .tiling import linear_weight_window, padded_batch_size, shard_rows, tile_st
 from .stages import coarse_stage_tile, decoder_stage_tile, latent_stage_tiles, process_latent_conditioning  # noqa: F401
 from .lazy_canvas import LazyCanvas, TensorWindow  # noqa: F401
 from .pipeline import TerrainPipeline, WorldPipeline  # noqa: F401
+from .relief import get_relief_map  # noqa: F401
 from .multiphase import (build_timestep_ranges, infinite_diffusion_canvases, phase_step_ranges,  # noqa: F401
                          sample_infinite_diffusion)

@@ -393,6 +393,15 @@ class WorldPipeline:
             return out
         return {k: (v.cpu() if torch.is_tensor(v) else v) for k, v in out.items()}
 
+    def get_relief(self, i1: int, j1: int, i2: int, j2: int, **kw):
+        """Shaded relief RGB [H, W, 3] of the elevation over pixel rows [i1,i2) x columns [j1,j2): `get_elev` and then
+        `get_relief_map` on the device, with `resolution` defaulting to `native_resolution` as the explorer passes it
+        (server.py:219-226).  numpy for WorldPipeline, a CUDA tensor for TerrainPipeline."""
+        from .relief import get_relief_map
+        kw.setdefault("resolution", self.native_resolution)
+        rgb = get_relief_map(self.get_elev(i1, j1, i2, j2), None, None, None, **kw)
+        return rgb.cpu().numpy() if self._host_views else rgb
+
     def residual_normalized(self, i1: int, j1: int, i2: int, j2: int) -> torch.Tensor:
         """Blended decoder output over pixel rows [i1,i2) x columns [j1,j2): residual[0] / residual[1] (on the device)."""
         r = self._residual[:, i1:i2, j1:j2]
