@@ -116,7 +116,7 @@ typedef struct TdxIm2colDesc {
   int32_t src_dtype[2];      /* 0 = fp32, 1 = bf16 */
   const float* src_scale[2]; /* optional DEVICE scalar multiplied into source i (precondition_inputs), or NULL */
   void* out;                 /* bf16 NC8HW8 [n_img][k_pad/8][H][W][8] */
-  int32_t k_pad;             /* 9 * (sum(src_channels) + 1) rounded up to a multiple of 64; sum = 5 or 11 */
+  int32_t k_pad;             /* 9 * (sum(src_channels) + 1) rounded up to a multiple of 64; sum = 1, 4, 5 or 11 */
   int32_t n_img, height, width;
 } TdxIm2colDesc;
 int tdx_im2col_run(const TdxIm2colDesc* desc, void* stream);

@@ -87,8 +87,8 @@ int im2col_validate(const TdxIm2colDesc& d) {
   TDX_REQUIRE(d.src_channels[1] == 0 || d.src[1], "im2col: src[1] missing");
   TDX_REQUIRE(d.out, "im2col: out is null");
   const int ci = d.src_channels[0] + d.src_channels[1] + 1;
-  TDX_REQUIRE(ci == 6 || ci == 12, "im2col: %d input channels; instantiated for 5 (decoder / latent models) or 11 "
-              "(coarse model)", ci - 1);
+  TDX_REQUIRE(ci == 2 || ci == 5 || ci == 6 || ci == 12, "im2col: %d input channels; instantiated for 1 (autoencoder "
+              "encoder), 4 (autoencoder decoder), 5 (decoder / latent models) or 11 (coarse model)", ci - 1);
   TDX_REQUIRE(d.k_pad == ((9 * ci + 63) / 64) * 64, "im2col: k_pad=%d must be 9*%d rounded up to a multiple of 64",
               d.k_pad, ci);
   TDX_REQUIRE(d.n_img >= 1 && d.n_img <= 65535 && d.height >= 1 && d.width >= 1, "im2col: bad shape");
@@ -112,7 +112,9 @@ int im2col_launch(const TdxIm2colDesc& d, cudaStream_t stream) {
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[1];
   fill_launch_config(&cfg, attr, grid, dim3(128), 0, stream);
-  if (p.ci == 6) TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, im2col_in_kernel<6>, p));
+  if (p.ci == 2) TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, im2col_in_kernel<2>, p));
+  else if (p.ci == 5) TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, im2col_in_kernel<5>, p));
+  else if (p.ci == 6) TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, im2col_in_kernel<6>, p));
   else TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, im2col_in_kernel<12>, p));
   return TDX_OK;
 }

@@ -1,6 +1,7 @@
 """Mirror of the sampling part of terrain_diffusion.inference / terrain_diffusion.training.evaluation."""
 from .canvas import BlendCanvas  # noqa: F401
-from .samplers import (sample_base_consistency, sample_base_diffusion, sample_coarse_tiled,  # noqa: F401
+from .samplers import (decode_autoencoder_latents_tiled, sample_autoencoder_tiled,  # noqa: F401
+                       sample_base_consistency, sample_base_diffusion, sample_coarse_tiled,
                        sample_decoder_consistency_tiled, sample_decoder_diffusion_sharded,
                        sample_decoder_diffusion_tiled)
 from .sharded import ShardedCanvas  # noqa: F401

@@ -421,3 +421,116 @@ def sample_decoder_diffusion_sharded(model, scheduler, cond_img: torch.Tensor, n
             canvas.start_exchange()          # boundary rows are done: their strip travels during the interior solves
     canvas.finalize()
     return canvas.normalized_owned(), (canvas.own_lo, canvas.own_hi)
+
+
+def _window(weight_window_fn, size: int, device) -> torch.Tensor:
+    """[size, size] fp32 blend weights: weight_window_fn(size, device, dtype) ([size, size] or [1, 1, size, size], as
+    the reference's window functions return) or the reference's linear window."""
+    if weight_window_fn is None:
+        return linear_weight_window(size, device).contiguous()
+    return weight_window_fn(size, device, torch.float32).to(device=device, dtype=torch.float32).reshape(size, size)
+
+
+@torch.no_grad()
+def sample_autoencoder_tiled(model, images: torch.Tensor, tile_size: Optional[int] = None,
+                             tile_stride: Optional[int] = None, *, cond_img: Optional[torch.Tensor] = None,
+                             conditional_inputs=None, use_mode: bool = False, weight_window_fn=None,
+                             tile_batch: Optional[int] = None):
+    """Tiled reconstruction with an EDMAutoencoder (training/evaluation/sample_autoencoder.py:8-58): per tile
+    preencode -> postencode -> decode, blended in row-major order; [B, out_channels, H, W] in images' dtype.
+
+    tile_size defaults to the image width, tile_stride to tile_size.  The tiles of `tile_batch` tiles (default: all)
+    go through one preencode and one decode call; with use_mode=False each tile still draws its own
+    randn_like(std) in row-major order, as the reference's per-tile postencode does.  tile_size must be a multiple of
+    64 (three 2x down-samplings to a multiple of 8) and fit in the image; otherwise ValueError before any device work."""
+    conditional_inputs = list(conditional_inputs or [])
+    b, _, h, w = images.shape
+    T = tile_size or w
+    stride = tile_stride or T
+    if T % 64 or T > h or T > w:
+        raise ValueError(f"tile_size {T} on a {h}x{w} image: the GPU path takes tiles that are multiples of 64 and fit "
+                         "in the image")
+    if model.config["direct_skips"]:
+        raise NotImplementedError("direct_skips is not implemented by the GPU path (no shipped autoencoder uses it)")
+    device, dtype = images.device, images.dtype
+    enc_in = images if cond_img is None else torch.cat([images, cond_img], dim=1)
+    enc_in = enc_in.to(model.device).float()
+    window = _window(weight_window_fn, T, model.device)
+    out_channels = int(model.config.get("out_channels") or images.shape[1])
+    tiles = [(i0, j0) for i0 in tile_starts(h, T, stride) for j0 in tile_starts(w, T, stride)]
+    canvas = [BlendCanvas(out_channels, h, w, model.device) for _ in range(b)]
+    group = len(tiles) if tile_batch is None else max(1, int(tile_batch))
+    for g0 in range(0, len(tiles), group):
+        chunk = tiles[g0:g0 + group]
+        k = len(chunk)
+        x = torch.cat([enc_in[..., i0:i0 + T, j0:j0 + T] for (i0, j0) in chunk], dim=0)
+        cond = [torch.cat([torch.as_tensor(c).to(model.device)] * k, dim=0) for c in conditional_inputs]
+        means, logvars = model.preencode(x, cond)
+        latent = torch.cat([model.postencode(means[q * b:(q + 1) * b], logvars[q * b:(q + 1) * b], use_mode=use_mode)
+                            for q in range(k)], dim=0)
+        out = model.decode(latent)
+        for q, (i0, j0) in enumerate(chunk):
+            for bi in range(b):
+                canvas[bi].accumulate(out[q * b + bi], i0, j0, window)
+    return torch.stack([cv.normalized() for cv in canvas]).to(device=device, dtype=dtype)
+
+
+def _latent_tile_geometry(lh: int, lw: int, tile_size: int, tile_stride: int) -> list:
+    """Tiles of decode_autoencoder_latents_tiled (sample_autoencoder.py:97-117): per tile (i0, j0, li0, lj0, i_off,
+    j_off) with the latent window [li0, li0 + ceil(tile/8)) clipped to the latents and the output offset
+    i0 - 8 * li0.  ValueError where the reference's slice assignment fails with a shape mismatch (a slice shorter than
+    the tile), and where the latent window is not a multiple of 8 (the decoder's kernels)."""
+    n_lat = math.ceil(tile_size / 8)
+    tiles = []
+    for i0 in tile_starts(lh * 8, tile_size, tile_stride):
+        for j0 in tile_starts(lw * 8, tile_size, tile_stride):
+            li0, lj0 = i0 // 8, j0 // 8
+            rows, cols = min(lh, li0 + n_lat) - li0, min(lw, lj0 + n_lat) - lj0
+            i_off, j_off = i0 - 8 * li0, j0 - 8 * lj0
+            if i0 + tile_size > lh * 8 or j0 + tile_size > lw * 8 or i_off + tile_size > 8 * rows or \
+                    j_off + tile_size > 8 * cols:
+                raise ValueError(f"tile_size {tile_size}, stride {tile_stride} on {lh}x{lw} latents: the tile at "
+                                 f"({i0}, {j0}) does not fit the decoded {8 * rows}x{8 * cols} latent window or the "
+                                 f"{lh * 8}x{lw * 8} output")
+            if rows % 8 or cols % 8:
+                raise ValueError(f"tile_size {tile_size}: latent windows of {rows}x{cols}; the GPU path decodes "
+                                 "latent tiles that are multiples of 8")
+            tiles.append((i0, j0, li0, lj0, i_off, j_off))
+    return tiles
+
+
+@torch.no_grad()
+def decode_autoencoder_latents_tiled(model, latents: torch.Tensor, tile_size: Optional[int] = None,
+                                     tile_stride: Optional[int] = None, *, weight_window_fn=None,
+                                     tile_batch: Optional[int] = None):
+    """Tiled decoding of latents with an EDMAutoencoder (training/evaluation/sample_autoencoder.py:61-119).
+
+    tile_size None decodes the whole tensor in one call.  Otherwise tile_size / tile_stride are in output pixels (8
+    per latent): each tile decodes the latents [i0 // 8, i0 // 8 + ceil(tile / 8)), clipped, and keeps the tile_size
+    pixels from offset i0 - 8 * (i0 // 8); tiles are blended in row-major order.  The latent windows of `tile_batch`
+    tiles (default: all) go through one decode call.  Geometries the reference cannot blend, or whose latent windows
+    are not multiples of 8, raise ValueError before any device work."""
+    b, _, lh, lw = latents.shape
+    if model.config["direct_skips"]:
+        raise NotImplementedError("direct_skips is not implemented by the GPU path (no shipped autoencoder uses it)")
+    if tile_size is None:
+        if lh % 8 or lw % 8:
+            raise ValueError(f"{lh}x{lw} latents: the GPU path decodes latents that are multiples of 8")
+        return model.decode(latents)
+    T = tile_size
+    tiles = _latent_tile_geometry(lh, lw, T, tile_stride or T)
+    device, dtype = latents.device, latents.dtype
+    lat = latents.to(model.device).float()
+    window = _window(weight_window_fn, T, model.device)
+    out_channels = int(model.config.get("out_channels") or model.config.get("in_channels") or 1)
+    canvas = [BlendCanvas(out_channels, lh * 8, lw * 8, model.device) for _ in range(b)]
+    n_lat = math.ceil(T / 8)
+    group = len(tiles) if tile_batch is None else max(1, int(tile_batch))
+    for g0 in range(0, len(tiles), group):
+        chunk = tiles[g0:g0 + group]
+        z = torch.cat([lat[..., li0:li0 + n_lat, lj0:lj0 + n_lat] for (_, _, li0, lj0, _, _) in chunk], dim=0)
+        out = model.decode(z)
+        for q, (i0, j0, _, _, io, jo) in enumerate(chunk):
+            for bi in range(b):
+                canvas[bi].accumulate(out[q * b + bi, :, io:io + T, jo:jo + T].contiguous(), i0, j0, window)
+    return torch.stack([cv.normalized() for cv in canvas]).to(device=device, dtype=dtype)

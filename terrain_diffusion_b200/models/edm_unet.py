@@ -90,8 +90,6 @@ class EDMUnet2D(nn.Module):
             conditional_inputs=conditional_inputs, encode_only=encode_only, disable_out_gain=disable_out_gain,
             fourier_scale=fourier_scale, n_logvar=n_logvar)
         cfg = self._internal_dict
-        if encode_only:
-            raise NotImplementedError("encode_only models are not part of the sampling hot path")
         self.concat_balance = concat_balance
         mults = model_channel_mults or [1, 2, 3, 4]
         emb_ch = emb_channels or model_channels * max(mults)
@@ -244,7 +242,7 @@ class EDMUnet2D(nn.Module):
                 x=torch.zeros((n, fw.in_channels, h, w), dtype=torch.float32, device=dev),
                 labels=torch.zeros((n,), dtype=torch.float32, device=dev),
                 emb=torch.zeros((n, fw.emb_channels), dtype=torch.float32, device=dev) if with_emb else None,
-                out=torch.zeros((n, fw.out_channels, h, w), dtype=torch.float32, device=dev))
+                out=torch.zeros((n, fw.out_channels, em.out_h, em.out_w), dtype=torch.float32, device=dev))
             prog = UNetProgram(dev)
             em.emit_embed(prog, labels=bufs.labels, emb_in=bufs.emb)
             em.emit(prog, [(bufs.x, fw.in_channels, None)], model_out=bufs.out)
@@ -264,15 +262,17 @@ class EDMUnet2D(nn.Module):
         if x.device.type != "cuda":
             raise L.TdxError("EDMUnet2D (GPU path) got a CPU tensor; there is no CPU fallback")
         n, c, h, w = x.shape
-        needs_host_emb = precomputed_embeds is not None or len(self.conditional_layers) > 0 or \
-            not (self.noise_fourier is not None and self.noise_fourier.positional)
+        # a model without an embedding (encode_only with no noise or conditional inputs) has no modulation vectors
+        needs_host_emb = self.emb_channels > 0 and (
+            precomputed_embeds is not None or len(self.conditional_layers) > 0 or
+            not (self.noise_fourier is not None and self.noise_fourier.positional))
         prog, bufs = self._forward_plan(n, h, w, needs_host_emb)
         bufs.x.copy_(x)
         if needs_host_emb:
             emb = precomputed_embeds if precomputed_embeds is not None else \
                 self._host_embedding(noise_labels, conditional_inputs)
             bufs.emb.copy_(emb)
-        else:
+        elif self.emb_channels > 0:
             bufs.labels.copy_(noise_labels.reshape(-1).expand(n) if noise_labels.numel() == 1 else noise_labels)
         prog.run(self.use_cuda_graph)
         out = bufs.out.to(x.dtype, copy=True)

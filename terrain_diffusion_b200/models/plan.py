@@ -29,6 +29,10 @@ from .. import _lib as L
 from ..layout import pack_weight_segments
 
 
+IM2COL_CHANNELS = (2, 5, 6, 12)
+"""Input channels + ones that tdx_im2col_run is instantiated for (csrc/tdx_direct.cu)."""
+
+
 def effective_weight(w: torch.Tensor, gain=1.0) -> torch.Tensor:
     """fp32 weight MPConv.forward convolves with (mp_layers.py:203-213): global-RMS normalise, gain / sqrt(fan_in)."""
     w = w.detach().to(torch.float32)
@@ -90,6 +94,37 @@ def block_plan(cfg: dict) -> tuple[list, list]:
     return enc, dec
 
 
+def autoencoder_decoder_plan(cfg: dict) -> tuple[list, list]:
+    """Module order / shapes of EDMAutoencoder's decoder (edm_autoencoder.py:86-103) in block_plan's form: the 1x1
+    `decoder_conv` over [z, ones] as the first convolution, then the `decoder.{i}` chain of decoder-mode blocks with no
+    skip concatenation (named by their index, so `dec.{i}.` is `decoder.{i}.`)."""
+    mults = cfg.get("model_channel_mults") or [1, 2, 3, 4]
+    mc = cfg.get("model_channels", 128)
+    lpb = cfg.get("layers_per_block_decoder") or cfg.get("layers_per_block", 3)
+    if isinstance(lpb, int):
+        lpb = [lpb] * len(mults)
+    attn_res = cfg.get("attn_resolutions") or []
+    cout = mc * mults[-1]
+    enc = [dict(name="conv", kind="conv", cin=cfg["latent_channels"] + 1, cout=cout)]
+    dec = []
+
+    def block(cin, c, resample="keep", attention=False):
+        dec.append(dict(name=str(len(dec)), kind="block", mode="dec", resample=resample, cin=cin, cout=c,
+                        attention=attention, concat=False))
+
+    for level, (ch, nb) in reversed(list(enumerate(zip([mc * m for m in mults], lpb)))):
+        res = cfg["image_size"] // 2 ** level
+        if level == len(mults) - 1:
+            block(cout, cout, attention=bool(cfg.get("midblock_attention", True)))
+            block(cout, cout)
+        else:
+            block(cout, cout, resample="up")
+        for _ in range(nb + 1):
+            block(cout, ch, attention=res in attn_res)
+            cout = ch
+    return enc, dec
+
+
 class FoldedWeights:
     """Device-resident effective weights of one model (fp32 small tensors + packed bf16 GEMM operands).
 
@@ -97,13 +132,15 @@ class FoldedWeights:
     on the fp32 master weights, done once: the results are uploaded with plain copies, so creating a model puts no
     kernel on the device (the reference re-normalises 130 tensors with ~7 launches each on EVERY forward)."""
 
-    def __init__(self, model, device):
+    def __init__(self, model, device, plan=None):
+        """model: anything with `.config` and `.state_dict()` named like EDMUnet2D's; plan: its (enc, dec) block lists
+        when they are not block_plan(model.config)."""
         cfg = dict(model.config)
         sd = {k: v.detach().cpu().to(torch.float32) for k, v in model.state_dict().items()}
         dev_arg, device = device, torch.device("cpu")      # fold on the host; upload at the end of __init__
         self.cfg = cfg
         self.device = device
-        enc, dec = block_plan(cfg)
+        enc, dec = block_plan(cfg) if plan is None else plan
         bk = cfg.get("block_kwargs") or {}
         for bad in ("conv_type", "resample_type", "activation", "no_padding", "expansion_factor"):
             if bk.get(bad) not in (None, "default", "pooling", "silu", False, 1):
@@ -158,10 +195,17 @@ class FoldedWeights:
             else:
                 g[f"cond{i}"] = sd[f"conditional_layers.{i}.weight"].contiguous()      # MPEmbedding: un-normalised table
         first = enc[0]
-        w_in = effective_weight(sd[f"enc.{first['name']}.weight"])               # [cout][ci][3][3]
+        w_in = effective_weight(sd[f"enc.{first['name']}.weight"])               # [cout][ci][3][3] or [cout][ci][1][1]
+        if w_in.shape[-1] == 1:
+            # a 1x1 first convolution (the autoencoder's decoder_conv) is the 3x3 one with zeros off the centre tap;
+            # padded after the fold, which normalises by the 1x1 fan-in
+            w_in = torch.nn.functional.pad(w_in, (1, 1, 1, 1))
         # the first convolution as the [cout][k_pad] matrix of its tensor-core path (tdx_im2col_run + 1x1 igemm):
         # k = tap * ci + c, zero-padded to a multiple of 64
         ci = w_in.shape[1]
+        if ci not in IM2COL_CHANNELS:
+            raise NotImplementedError(f"first convolution over {ci - 1} input channels (+ ones): the GPU path's im2col "
+                                      f"is instantiated for {', '.join(str(c - 1) for c in IM2COL_CHANNELS)}")
         self.conv_in_kpad = ((9 * ci + 63) // 64) * 64
         w_mat = torch.zeros((w_in.shape[0], self.conv_in_kpad, 1, 1), dtype=torch.float32, device=device)
         w_mat[:, :9 * ci, 0, 0] = w_in.permute(0, 2, 3, 1).reshape(w_in.shape[0], 9 * ci)
@@ -210,9 +254,11 @@ class FoldedWeights:
                         seg[p + "res1"] = [w1.bfloat16(), (ws[:, :cx] * (s1 * self.w_skip)).contiguous().bfloat16(),
                                            (ws[:, cx:] * (s2 * self.w_skip)).contiguous().bfloat16()]
                     else:
-                        assert ws is None, "decoder block without concat but with a skip conv is not planned"
                         seg[p + "res0"] = [w0.bfloat16()]
                         seg[p + "res1"] = [w1.bfloat16()]
+                        if ws is not None:
+                            # the autoencoder decoder's channel-changing blocks: conv_skip(x) joins res1 as a K-slab
+                            seg[p + "res1"].append((ws * self.w_skip).bfloat16())
         self.device = dev_arg
         for k in list(g):
             g[k] = g[k].to(dev_arg)
@@ -275,11 +321,13 @@ class UNetEmitter:
         """cvec_sets: how many independent label sets (e.g. solver steps) share this arena; the modulation vectors of
         all of them are produced by ONE embed launch (emit_embed) and selected per evaluation with `cvec_set`."""
         self.cvec_sets = cvec_sets
-        levels = len(fw.cfg.get("model_channel_mults") or [1, 2, 3, 4])
-        need = 8 * 2 ** (levels - 1)
+        downs = sum(b.get("resample") == "down" for b in fw.enc)
+        ups = sum(b.get("resample") == "up" for b in fw.dec)
+        need = 8 * 2 ** downs
         if h % need or w % need:
             raise ValueError(f"spatial size {h}x{w} must be a multiple of {need} for this model")
         self.fw, self.n, self.h, self.w = fw, n, h, w
+        self.out_h, self.out_w = h * 2 ** ups // 2 ** downs, w * 2 ** ups // 2 ** downs     # size of conv_out's output
         self.dev = fw.device
         self.arena: dict = {}
         self.cvecs: dict = {}
@@ -545,6 +593,8 @@ class UNetEmitter:
                 if b.get("concat"):
                     d = self._igemm(prog, [(hbuf, cout, 9), (cur["raw"], cx, 1), (sk["raw"], cs, 1)], key + "res1",
                                     cout, h, w)
+                elif b["cin"] != cout:
+                    d = self._igemm(prog, [(hbuf, cout, 9), (cur["raw"], b["cin"], 1)], key + "res1", cout, h, w)
                 else:
                     d = self._igemm(prog, [(hbuf, cout, 9)], key + "res1", cout, h, w)
                     d.epi_flags = L.EPI_RESID
