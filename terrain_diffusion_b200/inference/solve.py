@@ -132,9 +132,9 @@ class DiffusionSolve:
                 sched["guide_out"] = self.guide_out
             em.emit(self.prog, srcs, model_out=None, sched=sched, cvec_set=i)
         if self.guided:
-            # prog.arena stays the main model's activations (tools read it); the guide's is kept alive in prog.keep
+            # prog.arena / prog.cvecs stay the main model's (tools read them); the guide's are kept alive in prog.keep
             self.prog.keep.append(gem.arena)
-            self.prog.arena = em.arena
+            self.prog.arena, self.prog.cvecs = em.arena, em.cvecs
         self.launches_per_solve = self.prog.n_launch
 
     @torch.no_grad()

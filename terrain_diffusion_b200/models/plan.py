@@ -281,6 +281,7 @@ class UNetProgram:
         L.check(L.lib().tdx_program_create(C.byref(self.handle)))
         self.keep: list = []
         self.arena: dict = {}
+        self.cvecs: dict = {}
         self.n_igemm = 0
         self.n_launch = 0
 
@@ -622,3 +623,4 @@ class UNetEmitter:
         prog.add("conv_out", od)
         prog.keep.append((self.arena, self.cvecs, fw, srcs, model_out, sched))
         prog.arena = self.arena
+        prog.cvecs = self.cvecs
