@@ -17,10 +17,9 @@ from __future__ import annotations
 
 import torch
 
-from .canvas import BlendCanvas
 from .lazy_canvas import LazyCanvas, TensorWindow
 from .noise import gaussian_noise_patch
-from .samplers import get_diffusion_solve
+from .samplers import _blend_tiles, _gather, get_diffusion_solve
 from .tiling import linear_weight_window, tile_starts
 
 
@@ -77,21 +76,14 @@ def sample_infinite_diffusion(model, scheduler, cond_img: torch.Tensor, noise: t
     tiles = [(i0, j0) for i0 in tile_starts(h, tile_size, tile_stride) for j0 in tile_starts(w, tile_size, tile_stride)]
     cond32 = None if cond_img is None else cond_img.to(device).float()
     current = noise.float()
-    group = max(1, int(tile_batch))
     for rng in phase_step_ranges(scheduler, num_steps, thresholds):
-        canvases = [BlendCanvas(c, h, w, device) for _ in range(b)]
-        for g0 in range(0, len(tiles), group):
-            chunk = tiles[g0:g0 + group]
+        def run_group(chunk):
             solve = get_diffusion_solve(model, scheduler, b * len(chunk), tile_size, tile_size, num_steps,
                                         step_range=rng)
-            x = torch.cat([current[..., i0:i0 + tile_size, j0:j0 + tile_size] for (i0, j0) in chunk], dim=0)
-            cd = None if cond32 is None else torch.cat(
-                [cond32[..., i0:i0 + tile_size, j0:j0 + tile_size] for (i0, j0) in chunk], dim=0)
-            out = solve.run(x, cd)
-            for t, (i0, j0) in enumerate(chunk):
-                for bi in range(b):
-                    canvases[bi].accumulate(out[t * b + bi], i0, j0, window)
-        current = torch.stack([cv.normalized() for cv in canvases])       # what the next phase reads
+            cd = None if cond32 is None else _gather(cond32, chunk, tile_size)
+            return solve.run(_gather(current, chunk, tile_size), cd)
+
+        current = _blend_tiles(tiles, tile_batch, b, c, h, w, window, run_group)     # what the next phase reads
     return current.to(noise.dtype)
 
 

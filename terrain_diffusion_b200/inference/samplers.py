@@ -83,6 +83,37 @@ def get_consistency_solve(model, n, h, w, t: float, sigma_data: float = 0.5, fro
     return cache[key]
 
 
+def _window(weight_window_fn, size: int, device) -> torch.Tensor:
+    """[size, size] contiguous fp32 blend weights on `device`: weight_window_fn(size, device, dtype) ([size, size] or
+    [1, 1, size, size], as the reference's window functions return) or the reference's linear window."""
+    if weight_window_fn is None:
+        return linear_weight_window(size, device).contiguous()
+    w = weight_window_fn(size, device, torch.float32)
+    return w.to(device=device, dtype=torch.float32).reshape(size, size).contiguous()
+
+
+def _gather(x: torch.Tensor, chunk, size: int) -> torch.Tensor:
+    """The size x size windows of x at the (i0, j0, ...) tiles of `chunk`, concatenated on the batch axis."""
+    return torch.cat([x[..., i0:i0 + size, j0:j0 + size] for i0, j0, *_ in chunk], dim=0)
+
+
+def _blend_tiles(tiles, tile_batch: Optional[int], b: int, channels: int, height: int, width: int,
+                 window: torch.Tensor, run_group, divisor: float = 1.0) -> torch.Tensor:
+    """Solve `tiles` (row-major tuples that start with the tile origin (i0, j0)) in groups of `tile_batch` (None: all
+    in one group) and blend them in row-major order.  run_group(chunk) returns the chunk's outputs, [len(chunk) * b,
+    C, T, T] fp32 with the b images of a tile adjacent.  The b images share one canvas of b * C planes: every plane is
+    blended independently, so this is bit-identical to one canvas per image.  Returns the normalised [b, C, H, W]."""
+    canvas = BlendCanvas(b * channels, height, width, window.device)
+    t = window.shape[-1]
+    group = len(tiles) if tile_batch is None else max(1, int(tile_batch))
+    for g0 in range(0, len(tiles), group):
+        chunk = tiles[g0:g0 + group]
+        out = run_group(chunk)
+        for q, (i0, j0, *_) in enumerate(chunk):
+            canvas.accumulate(out[q * b:(q + 1) * b].reshape(b * channels, t, t), i0, j0, window)
+    return canvas.normalized(divisor).view(b, channels, height, width)
+
+
 @torch.no_grad()
 def sample_decoder_diffusion_tiled(model, scheduler, cond_img: torch.Tensor, noise: torch.Tensor,
                                    tile_size: Optional[int] = None, tile_stride: Optional[int] = None, *,
@@ -102,24 +133,16 @@ def sample_decoder_diffusion_tiled(model, scheduler, cond_img: torch.Tensor, noi
         cond_img = F.interpolate(cond_img, size=(h, w), mode="nearest")
     tile_size = tile_size or min(h, w)
     tile_stride = tile_stride or tile_size
-    window = (weight_window_fn(tile_size, device, torch.float32)[0, 0] if weight_window_fn is not None
-              else linear_weight_window(tile_size, device)).contiguous()
+    window = _window(weight_window_fn, tile_size, device)
     tiles = [(i0, j0) for i0 in tile_starts(h, tile_size, tile_stride) for j0 in tile_starts(w, tile_size, tile_stride)]
-    canvases = [BlendCanvas(c, h, w, device) for _ in range(b)]
     noise32, cond32 = noise.float(), cond_img.float()
-    group = max(1, int(tile_batch))
-    for g0 in range(0, len(tiles), group):
-        chunk = tiles[g0:g0 + group]
-        n = b * len(chunk)
-        solve = get_diffusion_solve(model, scheduler, n, tile_size, tile_size, num_steps, guide=guidance_model,
-                                    guidance_scale=guidance_scale, score_scaling=score_scaling)
-        x = torch.cat([noise32[..., i0:i0 + tile_size, j0:j0 + tile_size] for (i0, j0) in chunk], dim=0)
-        cd = torch.cat([cond32[..., i0:i0 + tile_size, j0:j0 + tile_size] for (i0, j0) in chunk], dim=0)
-        out = solve.run(x, cd)
-        for t, (i0, j0) in enumerate(chunk):
-            for bi in range(b):
-                canvases[bi].accumulate(out[t * b + bi], i0, j0, window)
-    return torch.stack([cv.normalized() for cv in canvases]).to(dtype)
+
+    def run_group(chunk):
+        solve = get_diffusion_solve(model, scheduler, b * len(chunk), tile_size, tile_size, num_steps,
+                                    guide=guidance_model, guidance_scale=guidance_scale, score_scaling=score_scaling)
+        return solve.run(_gather(noise32, chunk, tile_size), _gather(cond32, chunk, tile_size))
+
+    return _blend_tiles(tiles, tile_batch, b, c, h, w, window, run_group).to(dtype)
 
 
 def _reference_cond_vector(tile_cond, histogram_raw, cond_means, cond_stds, noise_level):
@@ -128,6 +151,23 @@ def _reference_cond_vector(tile_cond, histogram_raw, cond_means, cond_stds, nois
     from .stages import process_latent_conditioning
     return process_latent_conditioning(tile_cond, histogram_raw, cond_means, cond_stds, noise_level,
                                        reference_sampler_nans=True)
+
+
+def _base_tiles(cond_inputs, H: int, W: int, tile_size: int):
+    """(cond_inputs as a tensor, tiles) of the tiled base samplers: tiles of stride tile_size // 2 as (i0, j0, ic, jc),
+    where [ic:ic+4, jc:jc+4] is the tile's window of a 4-D condition image.  ValueError unless a condition image is
+    (len(starts)+3)-sized, and for a 1-D condition vector on more than one tile."""
+    stride = tile_size // 2
+    h_starts, w_starts = tile_starts(H, tile_size, stride), tile_starts(W, tile_size, stride)
+    cond_inputs = torch.as_tensor(cond_inputs)
+    if cond_inputs.ndim == 1 and len(h_starts) * len(w_starts) > 1:
+        raise ValueError(f"cond_inputs must be a tensor image for tiled sampling. Cond inputs must have width "
+                         f"{len(w_starts)+3} and height {len(h_starts)+3}.")
+    elif cond_inputs.ndim == 4:
+        if cond_inputs.shape[-1] != len(w_starts) + 3 or cond_inputs.shape[-2] != len(h_starts) + 3:
+            raise ValueError(f"cond_inputs is {tuple(cond_inputs.shape[-2:])}; tiled sampling of {H}x{W} needs "
+                             f"{len(h_starts)+3}x{len(w_starts)+3}")
+    return cond_inputs, [(i0, j0, ic, jc) for ic, i0 in enumerate(h_starts) for jc, j0 in enumerate(w_starts)]
 
 
 @torch.no_grad()
@@ -146,7 +186,6 @@ def sample_base_diffusion(model, scheduler, shape, cond_inputs, *, cond_means, c
 
     The initial noise is torch.randn(shape, generator=generator) * sigma_0 as the reference draws it; a CPU generator
     draws on the CPU and the noise is copied to the model's device."""
-    from .tiling import linear_weight_window as _lww
     device = model.device
     scheduler.set_timesteps(steps)
     sigma0 = float(scheduler.sigmas[0])      # sigma_max: the same for every step count
@@ -159,42 +198,26 @@ def sample_base_diffusion(model, scheduler, shape, cond_inputs, *, cond_means, c
         out = solve.run(noise.float(), None, conditional_inputs=[torch.as_tensor(c).to(device) for c in cond_inputs])
         return out.clone().to(dtype)
 
-    stride = tile_size // 2
-    h_starts, w_starts = tile_starts(H, tile_size, stride), tile_starts(W, tile_size, stride)
-    cond_inputs = torch.as_tensor(cond_inputs)
-    if cond_inputs.ndim == 1 and len(h_starts) * len(w_starts) > 1:
-        raise ValueError(f"cond_inputs must be a tensor image for tiled sampling. Cond inputs must have width "
-                         f"{len(w_starts)+3} and height {len(h_starts)+3}.")
-    elif cond_inputs.ndim == 4:
-        if cond_inputs.shape[-1] != len(w_starts) + 3 or cond_inputs.shape[-2] != len(h_starts) + 3:
-            raise ValueError(f"cond_inputs is {tuple(cond_inputs.shape[-2:])}; tiled sampling of {H}x{W} needs "
-                             f"{len(h_starts)+3}x{len(w_starts)+3}")
-    window = (weight_window_fn(tile_size, device, torch.float32)[0, 0] if weight_window_fn is not None
-              else _lww(tile_size, device)).contiguous()
-    tiles = [(ic, i0, jc, j0) for ic, i0 in enumerate(h_starts) for jc, j0 in enumerate(w_starts)]
-    # every tile's condition vector, in tile order (the reference computes them in this order too: the unseeded NaN
-    # fill draws from the global generator one tile after the other)
+    cond_inputs, grid = _base_tiles(cond_inputs, H, W, tile_size)
+    window = _window(weight_window_fn, tile_size, device)
+    # every tile carries its condition vector, computed in tile order (the reference computes them in this order too:
+    # the unseeded NaN fill draws from the global generator one tile after the other)
     if cond_inputs.ndim == 4:
         cimg = cond_inputs.to(device)
-        cvecs = [_reference_cond_vector(cimg[..., ic:ic + 4, jc:jc + 4], histogram_raw, cond_means, cond_stds,
-                                        noise_level) for ic, _, jc, _ in tiles]
+        tiles = [(i0, j0, _reference_cond_vector(cimg[..., ic:ic + 4, jc:jc + 4], histogram_raw, cond_means, cond_stds,
+                                                 noise_level)) for i0, j0, ic, jc in grid]
     else:
-        cvecs = [cond_inputs.to(device).float().reshape(1, -1).expand(B, -1)] * len(tiles)
-    canvas = [BlendCanvas(C, H, W, device) for _ in range(B)]
-    group = len(tiles) if tile_batch is None else max(1, int(tile_batch))
-    for g0 in range(0, len(tiles), group):
-        chunk = list(range(g0, min(g0 + group, len(tiles))))
+        fixed = cond_inputs.to(device).float().reshape(1, -1).expand(B, -1)
+        tiles = [(i0, j0, fixed) for i0, j0, _, _ in grid]
+
+    def run_group(chunk):
         solve = get_diffusion_solve(model, scheduler, B * len(chunk), tile_size, tile_size, steps, guide=guide_model,
                                     guidance_scale=guidance_scale)
-        x = torch.cat([noise[..., tiles[t][1]:tiles[t][1] + tile_size, tiles[t][3]:tiles[t][3] + tile_size]
-                       for t in chunk], dim=0).float()
-        cv = torch.cat([cvecs[t] for t in chunk], dim=0)
-        out = solve.run(x, None, conditional_inputs=[cv])
-        for k, t in enumerate(chunk):
-            for bi in range(B):
-                canvas[bi].accumulate(out[k * B + bi], tiles[t][1], tiles[t][3], window)
+        cv = torch.cat([cvec for _, _, cvec in chunk], dim=0)
+        return solve.run(_gather(noise, chunk, tile_size).float(), None, conditional_inputs=[cv])
+
     sd = float(scheduler.config.sigma_data)
-    return torch.stack([cv.normalized(sd) for cv in canvas]).to(dtype)
+    return _blend_tiles(tiles, tile_batch, B, C, H, W, window, run_group, sd).to(dtype)
 
 
 def _phase_times(scheduler, intermediate_t, dtype) -> list:
@@ -229,16 +252,7 @@ def sample_base_consistency(model, scheduler, shape, cond_inputs, *, cond_means,
     if tile_size is None:
         raise ValueError("sample_base_consistency samples in tiles: tile_size is required")
     B, C, H, W = shape
-    stride = tile_size // 2
-    h_starts, w_starts = tile_starts(H, tile_size, stride), tile_starts(W, tile_size, stride)
-    cond_inputs = torch.as_tensor(cond_inputs)
-    if cond_inputs.ndim == 1 and len(h_starts) * len(w_starts) > 1:
-        raise ValueError(f"cond_inputs must be a tensor image for tiled sampling. Cond inputs must have width "
-                         f"{len(w_starts)+3} and height {len(h_starts)+3}.")
-    elif cond_inputs.ndim == 4:
-        if cond_inputs.shape[-1] != len(w_starts) + 3 or cond_inputs.shape[-2] != len(h_starts) + 3:
-            raise ValueError(f"cond_inputs is {tuple(cond_inputs.shape[-2:])}; tiled sampling of {H}x{W} needs "
-                             f"{len(h_starts)+3}x{len(w_starts)+3}")
+    cond_inputs, grid = _base_tiles(cond_inputs, H, W, tile_size)
     if noise is not None and len(noise) < 1 + (intermediate_t > 0):
         raise ValueError(f"noise has {len(noise)} phases; this call runs {1 + (intermediate_t > 0)}")
     from .stages import trig_mix
@@ -246,10 +260,7 @@ def sample_base_consistency(model, scheduler, shape, cond_inputs, *, cond_means,
     sigma_data = float(scheduler.config.sigma_data)
     ts = _phase_times(scheduler, intermediate_t, dtype)
     T = tile_size
-    window = (weight_window_fn(T, device, torch.float32)[0, 0] if weight_window_fn is not None
-              else linear_weight_window(T, device)).contiguous()
-    tiles = [(ic, i0, jc, j0) for ic, i0 in enumerate(h_starts) for jc, j0 in enumerate(w_starts)]
-    group = len(tiles) if tile_batch is None else max(1, int(tile_batch))
+    window = _window(weight_window_fn, T, device)
     gen_dev = generator.device if generator is not None else device
     if cond_inputs.ndim == 4:
         cimg = cond_inputs.to(device)
@@ -263,26 +274,22 @@ def sample_base_consistency(model, scheduler, shape, cond_inputs, *, cond_means,
              else torch.as_tensor(noise[k]))
         z = z.to(device).float()
         if cond_inputs.ndim == 4:
-            cvecs = [_reference_cond_vector(cimg[..., ic:ic + 4, jc:jc + 4], histogram_raw, cond_means, cond_stds,
-                                            noise_level) for ic, _, jc, _ in tiles]
+            tiles = [(i0, j0, _reference_cond_vector(cimg[..., ic:ic + 4, jc:jc + 4], histogram_raw, cond_means,
+                                                     cond_stds, noise_level)) for i0, j0, ic, jc in grid]
         else:
-            cvecs = [fixed] * len(tiles)
-        canvas = [BlendCanvas(C, H, W, device) for _ in range(B)]
-        for g0 in range(0, len(tiles), group):
-            chunk = tiles[g0:g0 + group]
-            zt = torch.cat([z[..., i0:i0 + T, j0:j0 + T] for _, i0, _, j0 in chunk], dim=0).contiguous()
+            tiles = [(i0, j0, fixed) for i0, j0, _, _ in grid]
+
+        def run_group(chunk):
+            zt = _gather(z, chunk, T)
             if sample is None:
                 x = zt                                      # s = 0: x_t = sin t sigma_d z, folded into the program
             else:
-                st = torch.cat([sample[..., i0:i0 + T, j0:j0 + T] for _, i0, _, j0 in chunk], dim=0).contiguous()
-                x = trig_mix(st, zt, math.cos(t), math.sin(t) * sigma_data)
+                x = trig_mix(_gather(sample, chunk, T), zt, math.cos(t), math.sin(t) * sigma_data)
             solve = get_consistency_solve(model, B * len(chunk), T, T, t, sigma_data, from_unit_noise=sample is None)
-            out = solve.run(x, None, conditional_inputs=[torch.cat(cvecs[g0:g0 + len(chunk)], dim=0)])
-            for q, (_, i0, _, j0) in enumerate(chunk):
-                for bi in range(B):
-                    canvas[bi].accumulate(out[q * B + bi], i0, j0, window)
+            return solve.run(x, None, conditional_inputs=[torch.cat([cvec for _, _, cvec in chunk], dim=0)])
+
         last = k == len(ts) - 1
-        sample = torch.stack([cv.normalized(sigma_data if last else 1.0) for cv in canvas])
+        sample = _blend_tiles(tiles, tile_batch, B, C, H, W, window, run_group, sigma_data if last else 1.0)
     return sample.to(dtype)
 
 
@@ -328,31 +335,26 @@ def sample_coarse_tiled(model, scheduler, cond_img: torch.Tensor, cond_snr, *, s
     device, src = model.device, cond_img.device
     out_channels = int(model.config.get("out_channels") or model.config["in_channels"])
     T = tile_size
-    window = (weight_window_fn(T, device, torch.float32)[0, 0] if weight_window_fn is not None
-              else linear_weight_window(T, device)).contiguous()
+    window = _window(weight_window_fn, T, device)
     cond_inputs = [ci.to(device) for ci in cond_inputs_from_snr(cond_snr, src, dtype)]
     t_cond = torch.atan(cond_snr).view(1, -1, 1, 1).to(src)
     cond_img = torch.cos(t_cond) * cond_img + torch.sin(t_cond) * torch.randn_like(cond_img)
     scheduler.set_timesteps(int(steps))
     sigma0 = scheduler.sigmas[0].to(src)
-    tiles = [(i0, j0) for i0 in tile_starts(h, T, tile_stride) for j0 in tile_starts(w, T, tile_stride)]
-    noise = [(torch.randn((b, out_channels, T, T), device=src, generator=generator) * sigma0).to(device)
-             for _ in tiles]
+    # every tile carries its initial noise, drawn in row-major tile order
+    tiles = [(i0, j0, (torch.randn((b, out_channels, T, T), device=src, generator=generator) * sigma0).to(device))
+             for i0 in tile_starts(h, T, tile_stride) for j0 in tile_starts(w, T, tile_stride)]
     cond_d = cond_img.to(device).float()
     sd = float(scheduler.config.sigma_data)
-    canvas = [BlendCanvas(out_channels, h, w, device) for _ in range(b)]
-    group = len(tiles) if tile_batch is None else max(1, int(tile_batch))
-    for g0 in range(0, len(tiles), group):
-        chunk = tiles[g0:g0 + group]
+
+    def run_group(chunk):
         n = b * len(chunk)
         solve = get_diffusion_solve(model, scheduler, n, T, T, int(steps))
-        x = torch.cat(noise[g0:g0 + len(chunk)], dim=0).float()
-        cd = torch.cat([cond_d[..., i0:i0 + T, j0:j0 + T] for (i0, j0) in chunk], dim=0)
-        out = solve.run(x, cd, conditional_inputs=[ci.float().expand(n).contiguous() for ci in cond_inputs]) / sd
-        for q, (i0, j0) in enumerate(chunk):
-            for bi in range(b):
-                canvas[bi].accumulate(out[q * b + bi], i0, j0, window)
-    return torch.stack([cv.normalized() for cv in canvas]).to(device=src, dtype=dtype)
+        x = torch.cat([z for _, _, z in chunk], dim=0).float()
+        conds = [ci.float().expand(n).contiguous() for ci in cond_inputs]
+        return solve.run(x, _gather(cond_d, chunk, T), conditional_inputs=conds) / sd
+
+    return _blend_tiles(tiles, tile_batch, b, out_channels, h, w, window, run_group).to(device=src, dtype=dtype)
 
 
 @torch.no_grad()
@@ -368,8 +370,7 @@ def sample_decoder_consistency_tiled(model, scheduler, cond_img: torch.Tensor, n
         cond_img = F.interpolate(cond_img, size=(h, w), mode="nearest")
     tile_size = tile_size or min(h, w)
     tile_stride = tile_stride or tile_size
-    window = (weight_window_fn(tile_size, device, torch.float32)[0, 0] if weight_window_fn is not None
-              else linear_weight_window(tile_size, device)).contiguous()
+    window = _window(weight_window_fn, tile_size, device)
     sigma_data = float(scheduler.config.sigma_data)
     ts = [math.atan(float(scheduler.sigmas[0]) / sigma_data)]
     if intermediate_t is not None:
@@ -379,20 +380,21 @@ def sample_decoder_consistency_tiled(model, scheduler, cond_img: torch.Tensor, n
             ts += [float(v) for v in intermediate_t]
         else:
             ts.append(float(intermediate_t))
-    canvases = [BlendCanvas(c, h, w, device) for _ in range(b)]
-    for i0 in tile_starts(h, tile_size, tile_stride):
-        for j0 in tile_starts(w, tile_size, tile_stride):
-            samples = torch.zeros((b, c, tile_size, tile_size), device=device, dtype=torch.float32)
-            tile_cond = cond_img[..., i0:i0 + tile_size, j0:j0 + tile_size].float()
-            z = noise[..., i0:i0 + tile_size, j0:j0 + tile_size].float() * sigma_data
-            for t in ts:
-                x_t = math.cos(t) * samples + math.sin(t) * z
-                tt = torch.full((b,), t, device=device, dtype=torch.float32)
-                pred = -model(torch.cat([x_t / sigma_data, tile_cond], dim=1), tt, [])
-                samples = math.cos(t) * x_t - math.sin(t) * sigma_data * pred
-            for bi in range(b):
-                canvases[bi].accumulate(samples[bi].contiguous(), i0, j0, window)
-    return torch.stack([cv.normalized(sigma_data) for cv in canvases]).to(dtype)
+    tiles = [(i0, j0) for i0 in tile_starts(h, tile_size, tile_stride) for j0 in tile_starts(w, tile_size, tile_stride)]
+    noise32, cond32 = noise.float(), cond_img.float()
+
+    def run_group(chunk):
+        samples = torch.zeros((b, c, tile_size, tile_size), device=device, dtype=torch.float32)
+        tile_cond = _gather(cond32, chunk, tile_size)
+        z = _gather(noise32, chunk, tile_size) * sigma_data
+        for t in ts:
+            x_t = math.cos(t) * samples + math.sin(t) * z
+            tt = torch.full((b,), t, device=device, dtype=torch.float32)
+            pred = -model(torch.cat([x_t / sigma_data, tile_cond], dim=1), tt, [])
+            samples = math.cos(t) * x_t - math.sin(t) * sigma_data * pred
+        return samples
+
+    return _blend_tiles(tiles, 1, b, c, h, w, window, run_group, sigma_data).to(dtype)
 
 
 @torch.no_grad()
@@ -412,23 +414,13 @@ def sample_decoder_diffusion_sharded(model, scheduler, cond_img: torch.Tensor, n
     for g0 in range(0, len(tiles), group_n):
         chunk = tiles[g0:g0 + group_n]
         solve = get_diffusion_solve(model, scheduler, len(chunk), tile_size, tile_size, num_steps)
-        x = torch.cat([noise32[..., i0:i0 + tile_size, j0:j0 + tile_size] for (i0, j0) in chunk], dim=0)
-        cd = torch.cat([cond32[..., i0:i0 + tile_size, j0:j0 + tile_size] for (i0, j0) in chunk], dim=0)
-        out = solve.run(x, cd)
+        out = solve.run(_gather(noise32, chunk, tile_size), _gather(cond32, chunk, tile_size))
         for t, (i0, j0) in enumerate(chunk):
             canvas.add_tile(out[t].clone(), i0, j0)
         if g0 + len(chunk) >= canvas.n_boundary_tiles():
             canvas.start_exchange()          # boundary rows are done: their strip travels during the interior solves
     canvas.finalize()
     return canvas.normalized_owned(), (canvas.own_lo, canvas.own_hi)
-
-
-def _window(weight_window_fn, size: int, device) -> torch.Tensor:
-    """[size, size] fp32 blend weights: weight_window_fn(size, device, dtype) ([size, size] or [1, 1, size, size], as
-    the reference's window functions return) or the reference's linear window."""
-    if weight_window_fn is None:
-        return linear_weight_window(size, device).contiguous()
-    return weight_window_fn(size, device, torch.float32).to(device=device, dtype=torch.float32).reshape(size, size)
 
 
 @torch.no_grad()
@@ -458,21 +450,16 @@ def sample_autoencoder_tiled(model, images: torch.Tensor, tile_size: Optional[in
     window = _window(weight_window_fn, T, model.device)
     out_channels = int(model.config.get("out_channels") or images.shape[1])
     tiles = [(i0, j0) for i0 in tile_starts(h, T, stride) for j0 in tile_starts(w, T, stride)]
-    canvas = [BlendCanvas(out_channels, h, w, model.device) for _ in range(b)]
-    group = len(tiles) if tile_batch is None else max(1, int(tile_batch))
-    for g0 in range(0, len(tiles), group):
-        chunk = tiles[g0:g0 + group]
+
+    def run_group(chunk):
         k = len(chunk)
-        x = torch.cat([enc_in[..., i0:i0 + T, j0:j0 + T] for (i0, j0) in chunk], dim=0)
         cond = [torch.cat([torch.as_tensor(c).to(model.device)] * k, dim=0) for c in conditional_inputs]
-        means, logvars = model.preencode(x, cond)
+        means, logvars = model.preencode(_gather(enc_in, chunk, T), cond)
         latent = torch.cat([model.postencode(means[q * b:(q + 1) * b], logvars[q * b:(q + 1) * b], use_mode=use_mode)
                             for q in range(k)], dim=0)
-        out = model.decode(latent)
-        for q, (i0, j0) in enumerate(chunk):
-            for bi in range(b):
-                canvas[bi].accumulate(out[q * b + bi], i0, j0, window)
-    return torch.stack([cv.normalized() for cv in canvas]).to(device=device, dtype=dtype)
+        return model.decode(latent)
+
+    return _blend_tiles(tiles, tile_batch, b, out_channels, h, w, window, run_group).to(device=device, dtype=dtype)
 
 
 def _latent_tile_geometry(lh: int, lw: int, tile_size: int, tile_stride: int) -> list:
@@ -523,14 +510,12 @@ def decode_autoencoder_latents_tiled(model, latents: torch.Tensor, tile_size: Op
     lat = latents.to(model.device).float()
     window = _window(weight_window_fn, T, model.device)
     out_channels = int(model.config.get("out_channels") or model.config.get("in_channels") or 1)
-    canvas = [BlendCanvas(out_channels, lh * 8, lw * 8, model.device) for _ in range(b)]
     n_lat = math.ceil(T / 8)
-    group = len(tiles) if tile_batch is None else max(1, int(tile_batch))
-    for g0 in range(0, len(tiles), group):
-        chunk = tiles[g0:g0 + group]
-        z = torch.cat([lat[..., li0:li0 + n_lat, lj0:lj0 + n_lat] for (_, _, li0, lj0, _, _) in chunk], dim=0)
-        out = model.decode(z)
-        for q, (i0, j0, _, _, io, jo) in enumerate(chunk):
-            for bi in range(b):
-                canvas[bi].accumulate(out[q * b + bi, :, io:io + T, jo:jo + T].contiguous(), i0, j0, window)
-    return torch.stack([cv.normalized() for cv in canvas]).to(device=device, dtype=dtype)
+
+    def run_group(chunk):
+        out = model.decode(torch.cat([lat[..., li0:li0 + n_lat, lj0:lj0 + n_lat] for _, _, li0, lj0, _, _ in chunk]))
+        # each tile keeps the T x T pixels at its own offset in its decoded latent window
+        return torch.cat([out[q * b:(q + 1) * b, :, io:io + T, jo:jo + T] for q, (*_, io, jo) in enumerate(chunk)])
+
+    out = _blend_tiles(tiles, tile_batch, b, out_channels, lh * 8, lw * 8, window, run_group)
+    return out.to(device=device, dtype=dtype)

@@ -225,22 +225,25 @@ def test_consistency_multi_tile_matches_reference_golden(decoder):
 
 # ------------------------------------------------------------------------------------------------ blend
 def test_blend_canvas_is_bit_exact_with_oracle():
-    g = torch.Generator().manual_seed(12)
-    h, w, t, stride, c = 100, 148, 64, 48, 3
-    val = torch.zeros(1, c, h, w)
-    ws = torch.zeros(1, 1, h, w)
-    win = otile.linear_weight_window(t)
-    cv = BlendCanvas(c, h, w, "cuda")
-    for i0 in otile.tile_starts(h, t, stride):
-        for j0 in otile.tile_starts(w, t, stride):
-            tile = torch.randn(1, c, t, t, generator=g)
-            otile.accumulate(val, ws, tile, win[None, None], i0, j0)
-            cv.accumulate(tile[0].cuda(), i0, j0)
-    assert torch.equal(cv.val.cpu(), val[0])
-    assert torch.equal(cv.wsum.cpu(), ws[0, 0])
-    assert torch.equal(cv.normalized().cpu(), (val / ws)[0])
-    assert torch.equal(cv.normalized(0.5).cpu(), (val / ws / 0.5)[0])
-    assert torch.equal(cv.packed().cpu(), torch.cat([val[0], ws[0]], dim=0))
+    """One image, and a batch of b images on one canvas of b * C planes sharing one weight sum, as the tiled samplers
+    blend it."""
+    for b in (1, 3):
+        g = torch.Generator().manual_seed(12)
+        h, w, t, stride, c = 100, 148, 64, 48, 3
+        val = torch.zeros(b, c, h, w)
+        ws = torch.zeros(b, 1, h, w)
+        win = otile.linear_weight_window(t)
+        cv = BlendCanvas(b * c, h, w, "cuda")
+        for i0 in otile.tile_starts(h, t, stride):
+            for j0 in otile.tile_starts(w, t, stride):
+                tile = torch.randn(b, c, t, t, generator=g)
+                otile.accumulate(val, ws, tile, win[None, None], i0, j0)
+                cv.accumulate(tile.reshape(b * c, t, t).cuda(), i0, j0)
+        assert torch.equal(cv.val.cpu(), val.reshape(b * c, h, w)), b
+        assert torch.equal(cv.wsum.cpu(), ws[0, 0]), b
+        assert torch.equal(cv.normalized().cpu().view(b, c, h, w), val / ws), b
+        assert torch.equal(cv.normalized(0.5).cpu().view(b, c, h, w), val / ws / 0.5), b
+        assert torch.equal(cv.packed().cpu(), torch.cat([val.reshape(b * c, h, w), ws[0]], dim=0)), b
 
 
 def test_blend_canvas_negative_world_coordinates_and_clipping():
