@@ -291,6 +291,41 @@ int tdx_relief_shade(const float* elev, const float* blurred, const uint32_t* st
                      double cos_alt, float relief, float one_minus_relief, int32_t user_range, float vmin, float denom,
                      int32_t vmin_is_zero, float* out, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * River routing (d8_flow, flow_accumulation, plot_flow_indicator, inference/postprocessing.py:6-85), which the
+ * reference runs on the CPU, the accumulation as a Python loop over every land pixel.
+ * terrain_diffusion_b200/inference/hydrology.py composes the calls.  Elevations are contiguous fp32 [h][w] with h * w <= 2^24 (the largest size at
+ * which fp32 counts are exact); a pixel is ocean (invalid) when it is NaN or <= 0.  A pixel "pushes" when it is valid,
+ * not a sink and its receiver is valid; `recv` holds the receiver's flat index for those pixels and -1 elsewhere, and
+ * `indeg` the number of pixels that push into each pixel.  `flags` is a DEVICE uint32 the call zeroes and then ORs
+ * TDX_FLOW_* bits into.
+ * ------------------------------------------------------------------------------------------------------------------ */
+#define TDX_FLOW_INF 1            /* an elevation is +inf or -inf */
+#define TDX_FLOW_RANGE 2          /* a receiver index lies outside the image */
+#define TDX_FLOW_NOT_DOWNHILL 4   /* a followed edge is not strictly downhill in fp32 */
+/* d8_flow(z, tol) (postprocessing.py:6-46), bit for bit: neighbours N, S, W, E, NW, NE, SW, SE read edge-clamped,
+ * slope = (z - n) / dist in fp32, -inf where slope < tol (tol is the caller's fp32 rounding of the reference's
+ * argument), ocean rules, kmax = first argmax, is_sink, rr / cc = clamped receiver.  Each output may be NULL: kmax
+ * (int8), is_sink (uint8 0/1), rr and cc (int64), recv and indeg (in-degree gathered from the neighbours, no
+ * atomics).  Sets TDX_FLOW_INF.  With tol <= 0 a pixel may push to a neighbour of equal height or to itself; recv then
+ * does not describe a forest and must not be accumulated. */
+int tdx_flow_d8(const float* z, int32_t h, int32_t w, float tol, int8_t* kmax, uint8_t* is_sink, int64_t* rr,
+                int64_t* cc, int32_t* recv, uint32_t* indeg, uint32_t* flags, void* stream);
+/* recv and indeg from receivers given by the caller (flow_accumulation's rr, cc, is_sink: int64 / int64 / uint8
+ * [h][w]): sets TDX_FLOW_INF, TDX_FLOW_RANGE for any index outside the image, TDX_FLOW_NOT_DOWNHILL for a followed
+ * edge whose target is not strictly lower.  With no flag set, recv is a forest and may be accumulated. */
+int tdx_flow_link(const float* z, const int64_t* rr, const int64_t* cc, const uint8_t* is_sink, int32_t h, int32_t w,
+                  int32_t* recv, uint32_t* indeg, uint32_t* flags, void* stream);
+/* flow_accumulation (postprocessing.py:48-66) over the forest recv / indeg of z[n]: A = 1 + the sum of A over the
+ * pixels that push into it for valid pixels, 0 for invalid ones, as exact integers in fp32.  state: DEVICE uint64[n]
+ * scratch (zeroed by the call).  No thread waits on another. */
+int tdx_flow_accumulate(const float* z, int64_t n, const int32_t* recv, const uint32_t* indeg, uint64_t* state,
+                        float* A, void* stream);
+/* np.log1p of the non-overlapping k x k max-pool of A (remainder rows and columns dropped; k <= 1: no pool) into
+ * out[h / k][w / k] (postprocessing.py:72-85); nothing to do (out may be NULL) when that is empty.  A must be 0 at
+ * invalid pixels, as tdx_flow_accumulate leaves it. */
+int tdx_flow_indicator(const float* A, int32_t h, int32_t w, int32_t k, float* out, void* stream);
+
 /* Tile-seeded N(0,1) field, bit-exact with inference/portable_rng.py + world_pipeline.py:66-115 */
 int tdx_noise_patch(uint64_t base_seed, int64_t y0, int64_t x0, int32_t h, int32_t w, int32_t channels,
                     int32_t tile_h, int32_t tile_w, float* out, void* workspace, int64_t workspace_bytes,

@@ -154,6 +154,17 @@ def _declare(l: C.CDLL) -> None:
     l.tdx_relief_shade.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_float, C.c_float, C.c_double, C.c_double, C.c_double, C.c_float, C.c_float,
                                    C.c_int32, C.c_float, C.c_float, C.c_int32, C.c_void_p, C.c_void_p]
+    l.tdx_flow_d8.restype = C.c_int
+    l.tdx_flow_d8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
+                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    l.tdx_flow_link.restype = C.c_int
+    l.tdx_flow_link.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                C.c_void_p, C.c_void_p, C.c_void_p]
+    l.tdx_flow_accumulate.restype = C.c_int
+    l.tdx_flow_accumulate.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p]
+    l.tdx_flow_indicator.restype = C.c_int
+    l.tdx_flow_indicator.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     l.tdx_noise_patch.restype = C.c_int
     l.tdx_noise_patch.argtypes = [C.c_uint64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                   C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]

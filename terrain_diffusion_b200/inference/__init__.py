@@ -11,5 +11,6 @@ from .stages import coarse_stage_tile, decoder_stage_tile, latent_stage_tiles, p
 from .lazy_canvas import LazyCanvas, TensorWindow  # noqa: F401
 from .pipeline import TerrainPipeline, WorldPipeline  # noqa: F401
 from .relief import get_relief_map  # noqa: F401
+from .hydrology import d8_flow, flow_accumulation, plot_flow_indicator  # noqa: F401
 from .multiphase import (build_timestep_ranges, infinite_diffusion_canvases, phase_step_ranges,  # noqa: F401
                          sample_infinite_diffusion)
