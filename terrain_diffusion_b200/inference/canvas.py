@@ -34,11 +34,20 @@ class BlendCanvas:
         self.wsum.zero_()
 
     def accumulate(self, tile: torch.Tensor, y0: int, x0: int, window: torch.Tensor | None = None):
-        """tile: fp32 [C, T, T] on the canvas device; (y0, x0): world coordinates of its top-left pixel."""
+        """tile: fp32 [C, th, tw] on the canvas device; (y0, x0): world coordinates of its top-left pixel.  window: fp32
+        [th, tw] blend weights on the canvas device (any strides); None: the linear window, for square tiles only."""
         c, th, tw = tile.shape
         assert c == self.channels and tile.dtype == torch.float32 and tile.is_cuda
         tile = tile.contiguous()
-        win = self.window(th) if window is None else window
+        if window is None:
+            if th != tw:
+                raise ValueError(f"a {th}x{tw} tile needs an explicit [{th}, {tw}] window (the default is square)")
+            win = self.window(th)
+        else:
+            if tuple(window.shape) != (th, tw) or window.dtype != torch.float32 or window.device != self.val.device:
+                raise ValueError(f"window must be fp32 [{th}, {tw}] on {self.val.device}; got {window.dtype} "
+                                 f"{list(window.shape)} on {window.device}")
+            win = window.contiguous()
         L.call(L.lib().tdx_blend_accumulate, self.val.device, self.val.data_ptr(), self.wsum.data_ptr(), c, self.height,
                self.width, tile.data_ptr(), win.data_ptr(), th, tw, y0 - self.origin[0], x0 - self.origin[1])
 

@@ -199,6 +199,8 @@ class EDMDPMSolverMultistepScheduler:
         if self.num_inference_steps is None:
             raise ValueError(
                 "Number of inference steps is 'None', you need to run 'set_timesteps' after creating the scheduler")
+        if model_output.shape != sample.shape:       # the kernel reads sample.numel() elements of both
+            raise ValueError(f"model_output shape {list(model_output.shape)} != sample shape {list(sample.shape)}")
         if sample.device.type != "cuda":
             raise L.TdxError("scheduler.step (GPU path) needs CUDA tensors; there is no CPU fallback")
         if self._step_index is None:

@@ -122,6 +122,10 @@ def test_scheduler_tables_and_errors_on_cpu():
     with pytest.raises(ValueError):
         s.step(torch.zeros(1), torch.tensor(0.0), torch.zeros(1))
     s.set_timesteps(4)
+    for mo, x in ((torch.zeros(1), torch.zeros(2)), (torch.zeros(2, 3), torch.zeros(3, 2)),
+                  (torch.zeros(4), torch.zeros(1))):
+        with pytest.raises(ValueError, match="model_output shape"):       # before the device check
+            s.step(mo, s.timesteps[0], x)
     with pytest.raises(L.TdxError):
         s.step(torch.zeros(1), s.timesteps[0], torch.zeros(1))
     with pytest.raises(NotImplementedError):
