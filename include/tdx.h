@@ -242,7 +242,8 @@ int tdx_resize_aa_axis(const float* x, int32_t h, int32_t w, float* out, int32_t
 int tdx_gaussian_blur(const float* x, int32_t h, int32_t w, float* out, int32_t ksize, float sigma, void* stream);
 /* out[y][x] = f(a[y][x] + b[y][x]) over an h x w window of two pitched tensors (pass the pointers of the window's
  * first element): f = identity (laplacian_decode, laplacian_encoder.py:131) or sign(v) v^2 (world_pipeline.py:1312);
- * out_i16 (optional) additionally receives clip(floor(v), -32768, 32767) (api.py:73-77).  out or out_i16 may be NULL. */
+ * out_i16 (optional) additionally receives clip(floor(v), -32768, 32767) (api.py:73-77): +-inf pack as 32767 / -32768
+ * and NaN packs as 0, as numpy's float32 -> '<i2' cast does on x86.  out or out_i16 may be NULL. */
 int tdx_post_combine(const float* a, int64_t a_pitch, const float* b, int64_t b_pitch, float* out, int16_t* out_i16,
                      int32_t h, int32_t w, int32_t signed_square, void* stream);
 

@@ -169,8 +169,11 @@ def compute_elev(i1, j1, i2, j2, residual_planes, latents_planes, scale, residua
 
 
 def elev_to_int16(elev: np.ndarray) -> np.ndarray:
-    """api.py:73-77."""
-    return np.clip(np.floor(elev.astype(F32)), -32768, 32767).astype("<i2")
+    """api.py:73-77.  np.clip keeps a NaN, and numpy's float32 -> int16 cast of NaN is platform-defined: on x86 it goes
+    through cvttss2si (NaN -> 0x80000000) and keeps the low 16 bits, so NaN packs as 0.  That x86 result is the one pinned
+    here (explicitly, so the oracle gives it on any host) and in tdx_post_combine; +-inf clip to 32767 / -32768."""
+    f = np.floor(elev.astype(F32))
+    return np.clip(np.where(np.isnan(f), F32(0.0), f), -32768, 32767).astype("<i2")
 
 
 # ---------------------------------------------------------------------------------------------------- climate read-out

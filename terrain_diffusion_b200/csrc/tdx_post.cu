@@ -117,8 +117,9 @@ __global__ void post_combine_kernel(const float* __restrict__ a, long a_pitch, c
   if (signed_square) v = v == 0.f ? 0.f : copysignf(__fmul_rn(v, v), v);   // sign(v) * v^2 (world_pipeline.py:1312)
   if (out) out[(long)y * w + x] = v;
   if (out_i16) {
-    float f = floorf(v);                                                   // api.py:73-77: floor, clip, '<i2'
-    f = fminf(fmaxf(f, -32768.f), 32767.f);
+    // api.py:73-77: floor, clip, '<i2'.  numpy's clip keeps a NaN and its cast to int16 gives 0 on x86 (fmaxf would
+    // drop the NaN and pack -32768), so NaN packs as 0; +-inf clip to 32767 / -32768.
+    const float f = v != v ? 0.f : fminf(fmaxf(floorf(v), -32768.f), 32767.f);
     out_i16[(long)y * w + x] = (int16_t)f;
   }
 }
@@ -211,7 +212,8 @@ __global__ void climate_sample_kernel(const ClimateParams p) {
   const long cplane = (long)p.hc * p.wc;
   const float* central = p.coarse + (long)p.crop * p.wc + p.crop;
   const long plane = (long)p.h * p.w, o = (long)y * p.w + x;
-  p.out[o] = __fadd_rn(tb, __fmul_rn(be, fmaxf(p.elev[o], 0.0f)));
+  const float e = p.elev[o];                        // torch.maximum(elev, 0) keeps a NaN elevation (fmaxf would not)
+  p.out[o] = __fadd_rn(tb, __fmul_rn(be, e != e ? e : fmaxf(e, 0.0f)));
   p.out[plane + o] = sample(central + 3 * cplane, p.wc);
   p.out[2 * plane + o] = sample(central + 4 * cplane, p.wc);
   p.out[3 * plane + o] = sample(central + 5 * cplane, p.wc);

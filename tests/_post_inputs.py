@@ -54,6 +54,43 @@ def elev_canvases():
 def coarse_canvas():
     """Coarse canvas at 1/256 resolution: 6 value planes (0 = signed-sqrt elevation, 2 = temperature, ...) + weight."""
     c = FakeCanvas(3000, 6, (-12, -12), (30, 32), 0.0, 1.0)
-    c.val[0] = field(3100, 30, 32, 5.0, 18.0)        # signed sqrt of metres: mostly land, some ocean (< 0)
+    c.val[0] = field(3100, 30, 32, 5.0, 18.0)        # signed sqrt of metres: the windows ELEV_WINDOWS read are all land
     c.val[2] = field(3200, 30, 32, 12.0, 6.0)        # temperature, deg C
     return c
+
+
+# A coastal window at scale 2 (coarse stride 64): compute_climate reads coarse rows -11..10 and columns -12..11, and its
+# 15 x 15 lapse-rate windows give an 8 x 10 grid of regressions that take every branch of local_baseline_temperature.
+COASTAL_WINDOW, COASTAL_SCALE = (-150, -200, 170, 230), 2
+
+
+def coastal_canvas():
+    """Coarse canvas over exactly the rows / columns COASTAL_WINDOW reads: ocean (elevation < 0) everywhere except a
+    flat plateau (signed sqrt elevation exactly 1, so var_e < 1) in the top right and steep land in the bottom right
+    whose temperature rises with elevation in its top rows and falls fast in its bottom rows.  Windows to the left see
+    only ocean (den = 0), windows at the coast see a few land cells (den just below / above 0.02), and the regression
+    slopes overshoot both ends of beta_clip."""
+    c = FakeCanvas(4000, 6, (-11, -12), (22, 24), 0.0, 1.0)
+    e = -(0.5 + np.abs(field(4100, 22, 24)))
+    e[0:4, 17:] = 1.0
+    e[15:, 17:] = 4.0 + 14.0 * np.abs(field(4200, 7, 7))
+    t = field(4300, 22, 24, 12.0, 1.0)
+    t[15:17, 17:] = 5.0 + 0.02 * e[15:17, 17:] ** 2 + 0.1 * field(4400, 2, 7)
+    t[17:, 17:] = 25.0 - 0.1 * e[17:, 17:] ** 2 + 0.1 * field(4500, 5, 7)
+    c.val[0], c.val[2] = e.astype(np.float32), t.astype(np.float32)
+    return c
+
+
+def coastal_coarse_map():
+    """(temperature, signed-sqrt elevation) of the normalised coarse map compute_climate builds for COASTAL_WINDOW."""
+    i1, j1, i2, j2 = COASTAL_WINDOW
+    S = 32 * COASTAL_SCALE
+    c = coastal_canvas().planes(i1 // S - 8, -((-i2) // S) + 8, j1 // S - 8, -((-j2) // S) + 8).astype(np.float32)
+    cmap = (c[:-1] / c[-1:]).astype(np.float32)
+    return cmap[2], cmap[0]
+
+
+def coastal_elev():
+    """Elevation in metres over COASTAL_WINDOW (below sea level in places, so max(elev, 0) clamps)."""
+    i1, j1, i2, j2 = COASTAL_WINDOW
+    return field(4600, i2 - i1, j2 - j1, 100.0, 400.0)

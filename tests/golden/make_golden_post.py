@@ -2,9 +2,11 @@
 `terrain_diffusion/data/laplacian_encoder.py` is imported unchanged (it needs only torch + torchvision, both present in
 this container) and `WorldPipeline._compute_elev` is extracted from the reference source with `ast` and called with a
 stand-in `self` (world_pipeline.py itself cannot be imported: infinite_tensor, h5py, rasterio ... are absent).
-Only outputs are stored (tests/golden/post_golden.npz); inputs are regenerated from seeds by tests/_post_inputs.py.
+Only outputs are stored (tests/golden/post_golden.npz, and the coastal climate case in post_coastal_golden.npz); inputs
+are regenerated from seeds by tests/_post_inputs.py.
 
-    python tests/golden/make_golden_post.py
+    python tests/golden/make_golden_post.py            # both files
+    python tests/golden/make_golden_post.py coastal    # post_coastal_golden.npz only
 """
 from __future__ import annotations
 
@@ -25,8 +27,8 @@ sys.path[:0] = [str(ROOT / "oracle" / "_stub"), str(REF), str(ROOT)]
 
 from terrain_diffusion.data.laplacian_encoder import laplacian_decode, laplacian_denoise  # noqa: E402
 
-from tests._post_inputs import (ELEV_WINDOWS, RESIDUAL_MEAN, RESIDUAL_STD, coarse_canvas, elev_canvases,  # noqa: E402
-                                laplacian_case)
+from tests._post_inputs import (COASTAL_SCALE, COASTAL_WINDOW, ELEV_WINDOWS, RESIDUAL_MEAN, RESIDUAL_STD,  # noqa: E402
+                                coarse_canvas, coastal_canvas, coastal_elev, elev_canvases, laplacian_case)
 
 torch.set_grad_enabled(False)
 
@@ -40,15 +42,8 @@ class TorchCanvas:
         return torch.from_numpy(self.fake.planes(ys.start, ys.stop, xs.start, xs.stop).copy())
 
 
-def main():
-    out = {}
-    for name in ("rect", "square", "wide"):
-        r, l = laplacian_case(name)
-        r_t, l_t = torch.from_numpy(r), torch.from_numpy(l)
-        r2, l2 = laplacian_denoise(r_t, l_t, sigma=5)
-        out[f"lap_{name}_lowres"] = l2.numpy()
-        out[f"lap_{name}_elev"] = laplacian_decode(r2, l2).numpy()
-        out[f"lap_{name}_decode_extrap"] = laplacian_decode(r_t, l_t, extrapolate=True).numpy()
+def extract():
+    """WorldPipeline._compute_elev / _compute_climate and local_baseline_temperature_torch as plain functions."""
     src = (REF / "terrain_diffusion/inference/world_pipeline.py").read_text()
     tree = ast.parse(src)
     body = []
@@ -64,6 +59,18 @@ def main():
     import torch.nn.functional as F
     ns = {"torch": torch, "np": np, "F": F, "laplacian_denoise": laplacian_denoise, "laplacian_decode": laplacian_decode}
     exec(compile(ast.Module(body=body, type_ignores=[]), "world_pipeline_extract", "exec"), ns)
+    return ns
+
+
+def main(ns):
+    out = {}
+    for name in ("rect", "square", "wide"):
+        r, l = laplacian_case(name)
+        r_t, l_t = torch.from_numpy(r), torch.from_numpy(l)
+        r2, l2 = laplacian_denoise(r_t, l_t, sigma=5)
+        out[f"lap_{name}_lowres"] = l2.numpy()
+        out[f"lap_{name}_elev"] = laplacian_decode(r2, l2).numpy()
+        out[f"lap_{name}_decode_extrap"] = laplacian_decode(r_t, l_t, extrapolate=True).numpy()
     resid, lat = elev_canvases()
     fake = SimpleNamespace(kwargs={"residual_mean": RESIDUAL_MEAN, "residual_std": RESIDUAL_STD}, latents=TorchCanvas(lat),
                            coarse=TorchCanvas(coarse_canvas()))
@@ -77,5 +84,27 @@ def main():
     print("wrote", HERE / "post_golden.npz", sum(v.nbytes for v in out.values()) // 1024, "KiB raw")
 
 
+def coastal(ns):
+    """The coastal climate case (tests/_post_inputs.coastal_canvas) in a file of its own, so post_golden.npz stays as
+    recorded: the reference's local_baseline_temperature_torch on the normalised coarse map compute_climate builds, and
+    its _compute_climate over COASTAL_WINDOW (stored at every fourth pixel)."""
+    i1, j1, i2, j2 = COASTAL_WINDOW
+    cc = coastal_canvas()
+    fake = SimpleNamespace(coarse=TorchCanvas(cc))
+    S = 32 * COASTAL_SCALE
+    ci1, cj1, ci2, cj2 = i1 // S, j1 // S, -((-i2) // S), -((-j2) // S)
+    c = torch.from_numpy(cc.planes(ci1 - 8, ci2 + 8, cj1 - 8, cj2 + 8).copy())
+    cmap = c[:-1] / c[-1:]
+    e = torch.sign(cmap[0]) * torch.square(torch.maximum(torch.zeros_like(cmap[0]), cmap[0]))
+    t_sea, beta = ns["local_baseline_temperature_torch"](cmap[2], e, win=15, fallback_threshold=0.02)
+    clim = ns["_compute_climate"](fake, i1, j1, i2, j2, torch.from_numpy(coastal_elev()), COASTAL_SCALE)
+    out = {"t_sea": t_sea[0].numpy(), "beta": beta[0].numpy(), "climate": clim.numpy()[:, ::4, ::4]}
+    np.savez_compressed(HERE / "post_coastal_golden.npz", **out)
+    print("wrote", HERE / "post_coastal_golden.npz", sum(v.nbytes for v in out.values()) // 1024, "KiB raw")
+
+
 if __name__ == "__main__":
-    main()
+    extracted = extract()
+    if sys.argv[1:] != ["coastal"]:
+        main(extracted)
+    coastal(extracted)

@@ -7,10 +7,11 @@ import numpy as np
 import pytest
 
 from oracle import postproc as P
-from tests._post_inputs import (ELEV_WINDOWS, RESIDUAL_MEAN, RESIDUAL_STD, coarse_canvas, elev_canvases,
-                                laplacian_case)
+from tests._post_inputs import (COASTAL_SCALE, COASTAL_WINDOW, ELEV_WINDOWS, RESIDUAL_MEAN, RESIDUAL_STD, coarse_canvas,
+                                coastal_canvas, coastal_coarse_map, coastal_elev, elev_canvases, laplacian_case)
 
 G = np.load(Path(__file__).resolve().parent / "golden" / "post_golden.npz")
+GC = np.load(Path(__file__).resolve().parent / "golden" / "post_coastal_golden.npz")
 
 
 def rel(a, b):
@@ -80,6 +81,52 @@ def test_oracle_compute_climate_matches_reference_golden(name):
     for k in range(5):
         assert rel(c[k, ::2, ::2], g[k]) < 2e-6, k
     assert float(c[4].min()) >= -0.012 - 1e-9 and float(c[4].max()) <= 1e-9   # lapse rate stays inside beta_clip
+
+
+def test_coastal_lapse_rate_takes_every_branch_and_matches_reference_golden():
+    """The coastal coarse map runs every branch of local_baseline_temperature_torch (postprocessing.py:262-326) with
+    the thresholds _compute_climate passes: all-ocean windows (den = 0), land fractions 4/225 and 5/225 on either side
+    of fallback_threshold 0.02, flat land (var_e < 1) and slopes past both ends of beta_clip."""
+    T, c0 = coastal_coarse_map()
+    e = (np.sign(c0) * np.square(np.maximum(np.float32(0), c0))).astype(np.float32)     # world_pipeline.py:1329
+    t_sea, beta = P.local_baseline_temperature(T, e, 15, fallback_threshold=0.02)
+    assert rel(t_sea, GC["t_sea"]) < 2e-6 and np.array_equal(beta, GC["beta"])
+    F32 = np.float32
+    wm = (e > 0).astype(F32)
+    count = np.rint(P._avg_pool_valid(wm, 15) * 225).astype(int)
+    den = P._avg_pool_valid(wm, 15)
+
+    def wavg(x):
+        return (P._avg_pool_valid((x * wm).astype(F32), 15) / (den + F32(1e-6))).astype(F32)
+
+    mu_T, mu_e, mu_e2, mu_eT = wavg(T), wavg(e), wavg(e * e), wavg(e * T)
+    var_e = mu_e2 - mu_e ** 2
+    raw = (mu_eT - mu_e * mu_T) / (var_e + F32(1e-6))
+    valid = (var_e >= 1.0) & (den >= F32(0.02))
+    assert (count == 0).sum() >= 10 and (count == 4).any() and (count == 5).any()
+    assert ((den < F32(0.02)) & (count > 0)).sum() >= 3                 # sparse land falls back
+    assert ((var_e < 1.0) & (den >= F32(0.02))).sum() >= 3              # flat land falls back
+    assert (valid & (raw > 0.0)).sum() >= 3 and (valid & (raw < -0.012)).sum() >= 3      # clipped at both ends
+    assert ((den < F32(0.02)) | (var_e < 1.0)).sum() == (beta == F32(-0.0065)).sum()
+    assert set(np.unique(beta[valid])) <= {F32(0.0), F32(-0.012)}
+
+
+def test_oracle_coastal_climate_matches_reference_golden():
+    i1, j1, i2, j2 = COASTAL_WINDOW
+    c = P.compute_climate(i1, j1, i2, j2, coastal_elev(), coastal_canvas().planes, COASTAL_SCALE)
+    g = GC["climate"]                                      # stored at every fourth pixel
+    assert c.shape == (5, i2 - i1, j2 - j1)
+    for k in range(5):
+        assert rel(c[k, ::4, ::4], g[k]) < 2e-6, k
+
+
+def test_oracle_int16_packing_edges():
+    """api.py:73-77 (np.clip(np.floor(a), -32768, 32767).astype('<i2')) on x86 at the edges of the clip."""
+    a = np.array([np.nan, np.inf, -np.inf, -32768.5, -32769.0, 32767.9, 32768.0, -1e-30, -0.0, 0.0, 2.0 ** 23 + 1,
+                  -(2.0 ** 24), 1.5, -1.5], np.float32)
+    want = [0, 32767, -32768, -32768, -32768, 32767, 32767, -1, 0, 0, 32767, -32768, 1, -2]
+    got = P.elev_to_int16(a)
+    assert got.dtype == np.dtype("<i2") and got.tolist() == want
 
 
 def test_pipeline_get_wires_the_read_out_like_the_reference(monkeypatch):

@@ -1,6 +1,6 @@
 """Post step (elevation read-out) on the GPU: every tdx_post_* / tdx_resize_aa_axis / tdx_gaussian_blur primitive and
 their composition (terrain_diffusion_b200/inference/postproc.py) against the CPU oracle and against the golden vectors
-recorded from the reference (tests/golden/post_golden.npz).
+recorded from the reference (tests/golden/post_golden.npz, post_coastal_golden.npz).
 
 Tolerance: the kernels use the oracle's operation order with explicitly rounded fp32 operations, so primitives agree to
 a few ulp (rtol 2e-6 of the tensor's max); against the reference goldens 1e-5 (torch's conv sums in another order)."""
@@ -13,11 +13,12 @@ import torch
 from oracle import postproc as P
 from terrain_diffusion_b200 import _lib as L
 from terrain_diffusion_b200.inference import postproc as H
-from tests._post_inputs import (ELEV_WINDOWS, RESIDUAL_MEAN, RESIDUAL_STD, coarse_canvas, elev_canvases, field,
-                                laplacian_case)
+from tests._post_inputs import (COASTAL_SCALE, COASTAL_WINDOW, ELEV_WINDOWS, RESIDUAL_MEAN, RESIDUAL_STD,
+                                coarse_canvas, coastal_canvas, coastal_elev, elev_canvases, field, laplacian_case)
 
 pytestmark = pytest.mark.gpu
 G = np.load(Path(__file__).resolve().parent / "golden" / "post_golden.npz")
+GC = np.load(Path(__file__).resolve().parent / "golden" / "post_coastal_golden.npz")
 
 
 def rel(a, b):
@@ -106,3 +107,17 @@ def test_compute_climate_matches_reference_golden(name):
         assert rel(got[k, ::2, ::2], g[k]) < 1e-5, k
     with pytest.raises(ValueError):
         H.compute_climate(CudaCanvas(cc), i1, j1, i2 + 1, j2, dev(elev), 8)
+
+
+def test_compute_climate_coastal_matches_reference_golden():
+    """A coastal window at scale 2 whose lapse-rate regressions take every branch (all-ocean and sparse-land fallbacks,
+    flat land, both clip bounds): bit for bit against the oracle, and against the reference's own result."""
+    i1, j1, i2, j2 = COASTAL_WINDOW
+    cc, elev = coastal_canvas(), coastal_elev()
+    got = H.compute_climate(CudaCanvas(cc), i1, j1, i2, j2, dev(elev), COASTAL_SCALE).cpu().numpy()
+    ref = P.compute_climate(i1, j1, i2, j2, elev, cc.planes, COASTAL_SCALE)
+    assert got.shape == ref.shape == (5, i2 - i1, j2 - j1)
+    assert np.array_equal(got.view(np.uint32), ref.view(np.uint32))
+    g = GC["climate"]                                      # reference, stored at every fourth pixel
+    for k in range(5):
+        assert rel(got[k, ::4, ::4], g[k]) < 1e-5, k
