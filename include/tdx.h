@@ -246,6 +246,20 @@ int tdx_gaussian_blur(const float* x, int32_t h, int32_t w, float* out, int32_t 
  * and NaN packs as 0, as numpy's float32 -> '<i2' cast does on x86.  out or out_i16 may be NULL. */
 int tdx_post_combine(const float* a, int64_t a_pitch, const float* b, int64_t b_pitch, float* out, int16_t* out_i16,
                      int32_t h, int32_t w, int32_t signed_square, void* stream);
+/* The terrain API's read-out (api.py:103-166 _get_terrain, :73-100 _binary_response) in one pass.  Input: the padded
+ * native window elev [h][w] and optionally climate [5][h][w].  For scale >= 2 each output pixel (y, x) is torch's CPU
+ * F.interpolate(scale_factor=scale, mode='bilinear', align_corners=False) of the window at upsampled pixel
+ * (oi + y, oj + x), bit for bit, without building the upsampled planes: torch rounds two ways depending on the size of
+ * the whole upsampled window ((h + w) * scale <= 128 or not; both are restated in csrc/tdx_post.cu and
+ * oracle/terrain_api.py).  NaN results are the device's canonical NaN.  For scale == 1 the output is the window at
+ * (oi, oj) copied as is.  Outputs, each optional (at least one non-NULL):
+ *   elev_out [H][W] fp32, climate_out [5][H][W] fp32 (needs climate);
+ *   payload  the wire body: H*W int16-LE elevation (tdx_post_combine's packing: floor, clip, NaN -> 0) followed, when
+ *            climate is given, by H*W*4 fp32-LE climate channels 0..3 interleaved per pixel; 2-byte aligned.
+ * The crop must lie inside the upsampled window: oi + H <= h*scale, oj + W <= w*scale; H <= 65535. */
+int tdx_terrain_upsample(const float* elev, const float* climate, int32_t h, int32_t w, int32_t scale, int32_t oi,
+                         int32_t oj, int32_t H, int32_t W, float* elev_out, float* climate_out, void* payload,
+                         void* stream);
 
 /* Climate read-out (WorldPipeline._compute_climate, inference/world_pipeline.py:1314-1365).
  * tdx_lapse_rate = local_baseline_temperature_torch (inference/postprocessing.py:262-326) on the normalised coarse

@@ -106,6 +106,13 @@ __global__ void gaussian_blur_kernel(const float* __restrict__ x, int h, int w, 
   out[(long)oy * w + ox] = acc;
 }
 
+// api.py:73-77: floor, clip, '<i2'.  numpy's clip keeps a NaN and its cast to int16 gives 0 on x86 (fmaxf would drop
+// the NaN and pack -32768), so NaN packs as 0; +-inf clip to 32767 / -32768.
+__device__ __forceinline__ int16_t elev_to_i16(float v) {
+  const float f = v != v ? 0.f : fminf(fmaxf(floorf(v), -32768.f), 32767.f);
+  return (int16_t)f;
+}
+
 __global__ void post_combine_kernel(const float* __restrict__ a, long a_pitch, const float* __restrict__ b, long b_pitch,
                                     float* __restrict__ out, int16_t* __restrict__ out_i16, int h, int w,
                                     int signed_square) {
@@ -116,11 +123,86 @@ __global__ void post_combine_kernel(const float* __restrict__ a, long a_pitch, c
   float v = __fadd_rn(a[(long)y * a_pitch + x], b[(long)y * b_pitch + x]);
   if (signed_square) v = v == 0.f ? 0.f : copysignf(__fmul_rn(v, v), v);   // sign(v) * v^2 (world_pipeline.py:1312)
   if (out) out[(long)y * w + x] = v;
-  if (out_i16) {
-    // api.py:73-77: floor, clip, '<i2'.  numpy's clip keeps a NaN and its cast to int16 gives 0 on x86 (fmaxf would
-    // drop the NaN and pack -32768), so NaN packs as 0; +-inf clip to 32767 / -32768.
-    const float f = v != v ? 0.f : fminf(fmaxf(floorf(v), -32768.f), 32767.f);
-    out_i16[(long)y * w + x] = (int16_t)f;
+  if (out_i16) out_i16[(long)y * w + x] = elev_to_i16(v);
+}
+
+// The HTTP API's terrain read-out (api.py:103-166 _get_terrain + :80-100 _binary_response): torch's CPU
+// upsample_bilinear2d (align_corners=False, scale factor given) of the padded native window, evaluated only at the kept
+// output pixels, then the wire packing.  torch takes one of two CPU kernels by the size of the WHOLE upsampled window
+// (ATen UpSampleKernel.cpp, _use_vectorized_kernel_cond_2d: out_h + out_w <= 128 picks the per-pixel-weight kernel),
+// and the two round differently; both are restated here operation for operation (fma = the contraction x86 builds do):
+//   per axis:  src = max(fma(r, d + 0.5, -0.5), 0), r = fp32(1/scale);  i0 = min(floor(src), n-1), i1 = i0 + (i0 < n-1);
+//              l1 = clamp(src - i0, 0, 1), l0 = 1 - l1
+//   wide  (separable):   t_a = fma(wl0, x[a][j0], wl1 * x[a][j1]);  out = fma(hl0, t_i0, hl1 * t_i1)
+//   small (out_h + out_w <= 128):  w_ab = hl_a * wl_b;  out = fma(w11, x11, fma(w10, x10, fma(w00, x00, w01 * x01)))
+// scale == 1 is no interpolation at all (the reference returns get()'s window as is): a plain copy, so an inf does not
+// meet a zero weight.
+struct UpsampleParams {
+  const float* elev;      // [h][w]
+  const float* climate;   // [5][h][w] or NULL
+  float* elev_out;        // [H][W] or NULL
+  float* climate_out;     // [5][H][W] or NULL
+  uint16_t* payload;      // H*W int16 + H*W*4 fp32 (channels 0..3 interleaved), as 16-bit words, or NULL
+  int h, w, scale, oi, oj, H, W, small;
+  float r;
+};
+struct AxisTap {
+  int i0, i1;
+  float l0, l1;
+};
+__device__ __forceinline__ AxisTap upsample_axis(int d, int n, float r) {
+  const float src = fmaxf(__fmaf_rn(r, __fadd_rn((float)d, 0.5f), -0.5f), 0.0f);
+  AxisTap t;
+  t.i0 = min((int)floorf(src), n - 1);
+  t.i1 = t.i0 + (t.i0 < n - 1 ? 1 : 0);
+  t.l1 = fminf(fmaxf(__fsub_rn(src, (float)t.i0), 0.0f), 1.0f);
+  t.l0 = __fsub_rn(1.0f, t.l1);
+  return t;
+}
+__global__ void terrain_upsample_kernel(const UpsampleParams p) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+  if (x >= p.W || y >= p.H) return;
+  AxisTap ty, tx;
+  if (p.scale == 1) {
+    ty.i0 = ty.i1 = p.oi + y;
+    tx.i0 = tx.i1 = p.oj + x;
+  } else {
+    ty = upsample_axis(p.oi + y, p.h, p.r);
+    tx = upsample_axis(p.oj + x, p.w, p.r);
+  }
+  float w00 = 0.f, w01 = 0.f, w10 = 0.f, w11 = 0.f;
+  if (p.small) {
+    w00 = __fmul_rn(ty.l0, tx.l0); w01 = __fmul_rn(ty.l0, tx.l1);
+    w10 = __fmul_rn(ty.l1, tx.l0); w11 = __fmul_rn(ty.l1, tx.l1);
+  }
+  const long r0 = (long)ty.i0 * p.w, r1 = (long)ty.i1 * p.w;
+  auto sample = [&](const float* f) {
+    if (p.scale == 1) return f[r0 + tx.i0];
+    const float x00 = f[r0 + tx.i0], x01 = f[r0 + tx.i1], x10 = f[r1 + tx.i0], x11 = f[r1 + tx.i1];
+    if (p.small)
+      return __fmaf_rn(w11, x11, __fmaf_rn(w10, x10, __fmaf_rn(w00, x00, __fmul_rn(w01, x01))));
+    const float t0 = __fmaf_rn(tx.l0, x00, __fmul_rn(tx.l1, x01));
+    const float t1 = __fmaf_rn(tx.l0, x10, __fmul_rn(tx.l1, x11));
+    return __fmaf_rn(ty.l0, t0, __fmul_rn(ty.l1, t1));
+  };
+  const long o = (long)y * p.W + x, plane_in = (long)p.h * p.w, plane_out = (long)p.H * p.W;
+  const float e = sample(p.elev);
+  if (p.elev_out) p.elev_out[o] = e;
+  if (p.payload) p.payload[o] = (uint16_t)elev_to_i16(e);
+  if (!p.climate) return;
+  // channel 4 (the lapse rate) is in get_terrain's climate but not on the wire
+  const int n_ch = p.climate_out ? 5 : 4;
+  uint16_t* wire = p.payload ? p.payload + plane_out + 8 * o : nullptr;   // 2*H*W bytes in: only 2-byte aligned
+  for (int c = 0; c < n_ch; ++c) {
+    const float v = sample(p.climate + c * plane_in);
+    if (p.climate_out) p.climate_out[c * plane_out + o] = v;
+    if (wire && c < 4) {
+      const uint32_t bits = __float_as_uint(v);
+      wire[2 * c] = (uint16_t)(bits & 0xFFFFu);                            // little-endian fp32
+      wire[2 * c + 1] = (uint16_t)(bits >> 16);
+    }
   }
 }
 
@@ -300,6 +382,30 @@ extern "C" int tdx_post_combine(const float* a, int64_t a_pitch, const float* b,
   launch2d(&cfg, attr, h, w, reinterpret_cast<cudaStream_t>(stream));
   TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, post_combine_kernel, a, (long)a_pitch, b, (long)b_pitch, out, out_i16, (int)h,
                                     (int)w, (int)signed_square));
+  return TDX_OK;
+}
+
+extern "C" int tdx_terrain_upsample(const float* elev, const float* climate, int32_t h, int32_t w, int32_t scale,
+                                    int32_t oi, int32_t oj, int32_t H, int32_t W, float* elev_out, float* climate_out,
+                                    void* payload, void* stream) {
+  TDX_REQUIRE(elev && (elev_out || climate_out || payload), "terrain_upsample: null input or no output");
+  TDX_REQUIRE(!climate_out || climate, "terrain_upsample: climate_out without a climate window");
+  TDX_REQUIRE(((uintptr_t)payload & 1) == 0, "terrain_upsample: payload must be 2-byte aligned");
+  TDX_REQUIRE(scale >= 1 && h >= 1 && w >= 1 && H >= 1 && W >= 1 && H <= 65535,
+              "terrain_upsample: bad shape %d x %d x%d -> %d x %d", h, w, scale, H, W);
+  TDX_REQUIRE(oi >= 0 && oj >= 0 && (int64_t)oi + H <= (int64_t)h * scale && (int64_t)oj + W <= (int64_t)w * scale,
+              "terrain_upsample: crop %d x %d at (%d, %d) outside the %d x %d upsampled window", H, W, oi, oj, h * scale,
+              w * scale);
+  UpsampleParams p;
+  p.elev = elev; p.climate = climate; p.elev_out = elev_out; p.climate_out = climate_out;
+  p.payload = static_cast<uint16_t*>(payload);
+  p.h = h; p.w = w; p.scale = scale; p.oi = oi; p.oj = oj; p.H = H; p.W = W;
+  p.small = ((int64_t)h + w) * scale <= 128;
+  p.r = (float)(1.0 / scale);                          // compute_scales_value: static_cast<float>(1.0 / scale)
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  launch2d(&cfg, attr, H, W, reinterpret_cast<cudaStream_t>(stream));
+  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, terrain_upsample_kernel, p));
   return TDX_OK;
 }
 

@@ -393,6 +393,34 @@ class WorldPipeline:
             return out
         return {k: (v.cpu() if torch.is_tensor(v) else v) for k, v in out.items()}
 
+    def get_terrain(self, i1: int, j1: int, i2: int, j2: int, scale: int = 1, with_climate: bool = True) -> dict:
+        """The HTTP API's `_get_terrain` (api.py:103-166): {'elev': fp32 [H, W], 'climate': fp32 [5, H, W] | None} over
+        rows [i1, i2) x columns [j1, j2) of the world upsampled `scale` times (H = i2 - i1, W = j2 - j1).  The native
+        window padded by one pixel is computed on the device and upsampled there, bit for bit with the reference's
+        torch CPU bilinear interpolation, at the kept pixels only.  CPU tensors (one pinned copy) for WorldPipeline,
+        CUDA tensors for TerrainPipeline.
+
+        Raises ValueError for a non-integer argument, scale < 1 or an empty window at every scale (the reference
+        raises for an empty window only at scale 1 and returns wrongly sliced tensors above it)."""
+        from . import postproc
+        ni1, nj1, ni2, nj2, oi, oj = postproc.terrain_window(i1, j1, i2, j2, scale)
+        native = self._get_device(ni1, nj1, ni2, nj2, with_climate)
+        out = postproc.upsample_crop(native["elev"], native["climate"], int(scale), oi, oj, i2 - i1, j2 - j1)
+        if self._host_views:
+            out = postproc.to_host(out)
+        return {"elev": out[0], "climate": out[1:] if with_climate else None}
+
+    def terrain_payload(self, i1: int, j1: int, i2: int, j2: int, scale: int = 1) -> tuple:
+        """(body, (H, W)) of `GET /terrain` (api.py:174-201): body is `_binary_response(**_get_terrain(...))`'s, byte for
+        byte -- int16-LE elevation (floor, clip; NaN packs as 0) followed by climate channels 0..3 as fp32-LE interleaved
+        per pixel.  Packed on the device and copied to the host once.  Argument errors as get_terrain."""
+        from . import postproc
+        ni1, nj1, ni2, nj2, oi, oj = postproc.terrain_window(i1, j1, i2, j2, scale)
+        native = self._get_device(ni1, nj1, ni2, nj2, True)
+        H, W = i2 - i1, j2 - j1
+        body = postproc.upsample_crop(native["elev"], native["climate"], int(scale), oi, oj, H, W, payload=True)
+        return postproc.to_host(body).numpy().tobytes(), (H, W)
+
     def get_relief(self, i1: int, j1: int, i2: int, j2: int, **kw):
         """Shaded relief RGB [H, W, 3] of the elevation over pixel rows [i1,i2) x columns [j1,j2): `get_elev` and then
         `get_relief_map` on the device, with `resolution` defaulting to `native_resolution` as the explorer passes it

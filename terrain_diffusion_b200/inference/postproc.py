@@ -13,6 +13,7 @@ import ctypes as C
 
 import functools
 
+import numpy as np
 import torch
 
 from .. import _lib as L
@@ -172,6 +173,67 @@ def compute_elev(residual_canvas, latents_canvas, i1: int, j1: int, i2: int, j2:
     oi, oj = i1 - pi1, j1 - pj1
     h, w = i2 - i1, j2 - j1
     return _combine(residual_p[oi:oi + h, oj:oj + w], up[oi:oi + h, oj:oj + w], signed_square=True, int16=as_int16)
+
+
+def terrain_window(i1: int, j1: int, i2: int, j2: int, scale: int):
+    """Checks the arguments of a terrain request (api.py:68-69, 193-194) and returns the native window `_get_terrain`
+    reads and the crop origin in its upsampled version (api.py:114-153): (ni1, nj1, ni2, nj2, oi, oj).  The window is
+    padded by one native pixel on every side for scale > 1; Python floor / ceil division, so negative coordinates work.
+
+    Raises ValueError for a non-integer coordinate or scale, scale < 1, an empty window (i2 <= i1 or j2 <= j1) or more
+    than 65535 output rows.  The reference raises for an empty window only at scale 1; above it, it returns wrongly
+    sliced tensors."""
+    for name, v in (("i1", i1), ("j1", j1), ("i2", i2), ("j2", j2), ("scale", scale)):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+            raise ValueError(f"{name} must be an int, got {v!r}")
+    i1, j1, i2, j2, scale = int(i1), int(j1), int(i2), int(j2), int(scale)
+    if scale < 1:
+        raise ValueError("scale must be >= 1")
+    if i2 <= i1 or j2 <= j1:
+        raise ValueError("Expected i2>i1 and j2>j1")
+    if i2 - i1 > 65535:
+        raise ValueError(f"at most 65535 rows per request, got {i2 - i1}")
+    if scale == 1:
+        return i1, j1, i2, j2, 0, 0
+    ni1, nj1 = i1 // scale, j1 // scale
+    ni2, nj2 = -(-i2 // scale), -(-j2 // scale)
+    return ni1 - 1, nj1 - 1, ni2 + 1, nj2 + 1, scale + (i1 - ni1 * scale), scale + (j1 - nj1 * scale)
+
+
+@_on_arg_device
+def upsample_crop(elev: torch.Tensor, climate: torch.Tensor | None, scale: int, oi: int, oj: int, H: int, W: int,
+                  payload: bool = False) -> torch.Tensor:
+    """The terrain API's upsample + crop (api.py:139-164, torch's CPU F.interpolate(scale_factor=scale, mode='bilinear',
+    align_corners=False) bit for bit) of the native window `elev` [h, w] (and `climate` [5, h, w]), output pixels
+    [oi, oi+H) x [oj, oj+W) of the upsampled window only; scale == 1 is the plain crop.  Returns one CUDA tensor: fp32
+    [6, H, W] (elevation, then the 5 climate planes) or [1, H, W] without climate; with `payload`, the wire body of
+    api.py:80-100 as uint8 [2HW (+ 16HW with climate)]."""
+    elev = _chk(elev, "upsample_crop(elev)")
+    h, w = elev.shape
+    if climate is not None:
+        if not (isinstance(climate, torch.Tensor) and climate.is_cuda and climate.dtype == torch.float32
+                and tuple(climate.shape) == (5, h, w) and climate.device == elev.device):
+            raise L.TdxError(f"upsample_crop: climate must be a CUDA float32 [5, {h}, {w}] tensor on {elev.device}")
+        climate = climate.contiguous()
+    s = L.current_stream_ptr()
+    clim_p = _p(climate) if climate is not None else None
+    if payload:
+        out = torch.empty((H * W * (18 if climate is not None else 2),), dtype=torch.uint8, device=elev.device)
+        L.check(L.lib().tdx_terrain_upsample(_p(elev), clim_p, h, w, scale, oi, oj, H, W, None, None, _p(out), s))
+        return out
+    out = torch.empty((6 if climate is not None else 1, H, W), dtype=torch.float32, device=elev.device)
+    L.check(L.lib().tdx_terrain_upsample(_p(elev), clim_p, h, w, scale, oi, oj, H, W, _p(out[0]),
+                                         _p(out[1]) if climate is not None else None, None, s))
+    return out
+
+
+@_on_arg_device
+def to_host(t: torch.Tensor) -> torch.Tensor:
+    """One device -> host copy into pinned memory (torch's caching host allocator), on the current stream, waited for."""
+    staging = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
+    staging.copy_(t, non_blocking=True)
+    torch.cuda.current_stream(t.device).synchronize()
+    return staging
 
 
 @_on_arg_device
