@@ -260,6 +260,25 @@ int tdx_post_combine(const float* a, int64_t a_pitch, const float* b, int64_t b_
 int tdx_terrain_upsample(const float* elev, const float* climate, int32_t h, int32_t w, int32_t scale, int32_t oi,
                          int32_t oj, int32_t H, int32_t W, float* elev_out, float* climate_out, void* payload,
                          void* stream);
+/* The Minecraft API's read-out (minecraft_api.py:265-355 _get_upsampled, :189-263 _compute_climate_vars, :358-688
+ * _classify_biome, :90-99 _binary_response) in one pass over the H x W output pixels.
+ *   scale >= 2: elev [h][w] and climate [5][h][w] are the native window padded by 2 pixels; each pixel and its 1-pixel
+ *     ring are torch's CPU bilinear upsample of it at (oi + y, oj + x), bit for bit (the kernel is picked by the whole
+ *     upsampled window, (h + w) * scale <= 128); centre must be NULL.
+ *   scale == 1: elev is the slope window [H+2][W+2] with oi = oj = 1, centre the [H][W] window the pixel's elevation is
+ *     read from, climate [5][H][W]; detail must be 0.
+ * noise [5][H][W] holds the injected noise planes (temp/snow coarse, temp/snow fine, precip, elev coarse, elev fine);
+ * needed with climate or detail.  detail != 0 adds the slope-scaled detail noise with the fp32 scalars the reference's
+ * torch ops use: amp_c = fp32(noise * 100), amp_f = fp32(noise * 70), pixel_size_m, native_res and slope_div =
+ * fp32(40 * pixel_size_m / 90) (pixel_size_m also divides the slope for the classifier).  NULL climate: every id is 1.
+ * Outputs, each optional (at least one non-NULL): elev_out (with detail noise) and smooth_out [H][W] fp32,
+ * climate_out [5][H][W] fp32 (the upsampled planes, before noise), biome_out [H][W] int16, payload (int16-LE elevation,
+ * packed as tdx_post_combine, then int16-LE biome ids; 2-byte aligned). */
+int tdx_minecraft_readout(const float* elev, int32_t h, int32_t w, int32_t scale, int32_t oi, int32_t oj,
+                          const float* centre, const float* climate, const float* noise, int32_t H, int32_t W,
+                          int32_t detail, float amp_c, float amp_f, float pixel_size_m, float native_res,
+                          float slope_div, float* elev_out, float* smooth_out, float* climate_out, int16_t* biome_out,
+                          void* payload, void* stream);
 
 /* Climate read-out (WorldPipeline._compute_climate, inference/world_pipeline.py:1314-1365).
  * tdx_lapse_rate = local_baseline_temperature_torch (inference/postprocessing.py:262-326) on the normalised coarse

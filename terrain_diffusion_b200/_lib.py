@@ -141,6 +141,11 @@ def _declare(l: C.CDLL) -> None:
     l.tdx_terrain_upsample.restype = C.c_int
     l.tdx_terrain_upsample.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                        C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    l.tdx_minecraft_readout.restype = C.c_int
+    l.tdx_minecraft_readout.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float,
+                                        C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_void_p]
     l.tdx_lapse_rate.restype = C.c_int
     l.tdx_lapse_rate.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_float,
                                  C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]

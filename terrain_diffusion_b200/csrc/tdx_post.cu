@@ -7,6 +7,7 @@
 // pinned against the reference), so results agree to float32 round-off.  HBM-bound and tiny (a few hundred KB per call).
 #include "tdx_common.h"
 #include "tdx_ptx.cuh"
+#include "tdx_upsample.cuh"
 
 namespace tdx {
 
@@ -106,13 +107,6 @@ __global__ void gaussian_blur_kernel(const float* __restrict__ x, int h, int w, 
   out[(long)oy * w + ox] = acc;
 }
 
-// api.py:73-77: floor, clip, '<i2'.  numpy's clip keeps a NaN and its cast to int16 gives 0 on x86 (fmaxf would drop
-// the NaN and pack -32768), so NaN packs as 0; +-inf clip to 32767 / -32768.
-__device__ __forceinline__ int16_t elev_to_i16(float v) {
-  const float f = v != v ? 0.f : fminf(fmaxf(floorf(v), -32768.f), 32767.f);
-  return (int16_t)f;
-}
-
 __global__ void post_combine_kernel(const float* __restrict__ a, long a_pitch, const float* __restrict__ b, long b_pitch,
                                     float* __restrict__ out, int16_t* __restrict__ out_i16, int h, int w,
                                     int signed_square) {
@@ -128,15 +122,9 @@ __global__ void post_combine_kernel(const float* __restrict__ a, long a_pitch, c
 
 // The HTTP API's terrain read-out (api.py:103-166 _get_terrain + :80-100 _binary_response): torch's CPU
 // upsample_bilinear2d (align_corners=False, scale factor given) of the padded native window, evaluated only at the kept
-// output pixels, then the wire packing.  torch takes one of two CPU kernels by the size of the WHOLE upsampled window
-// (ATen UpSampleKernel.cpp, _use_vectorized_kernel_cond_2d: out_h + out_w <= 128 picks the per-pixel-weight kernel),
-// and the two round differently; both are restated here operation for operation (fma = the contraction x86 builds do):
-//   per axis:  src = max(fma(r, d + 0.5, -0.5), 0), r = fp32(1/scale);  i0 = min(floor(src), n-1), i1 = i0 + (i0 < n-1);
-//              l1 = clamp(src - i0, 0, 1), l0 = 1 - l1
-//   wide  (separable):   t_a = fma(wl0, x[a][j0], wl1 * x[a][j1]);  out = fma(hl0, t_i0, hl1 * t_i1)
-//   small (out_h + out_w <= 128):  w_ab = hl_a * wl_b;  out = fma(w11, x11, fma(w10, x10, fma(w00, x00, w01 * x01)))
-// scale == 1 is no interpolation at all (the reference returns get()'s window as is): a plain copy, so an inf does not
-// meet a zero weight.
+// output pixels (tdx_upsample.cuh: both of torch's kernels, picked by the size of the whole upsampled window), then the
+// wire packing.  scale == 1 is no interpolation at all (the reference returns get()'s window as is): a plain copy, so
+// an inf does not meet a zero weight.
 struct UpsampleParams {
   const float* elev;      // [h][w]
   const float* climate;   // [5][h][w] or NULL
@@ -146,19 +134,6 @@ struct UpsampleParams {
   int h, w, scale, oi, oj, H, W, small;
   float r;
 };
-struct AxisTap {
-  int i0, i1;
-  float l0, l1;
-};
-__device__ __forceinline__ AxisTap upsample_axis(int d, int n, float r) {
-  const float src = fmaxf(__fmaf_rn(r, __fadd_rn((float)d, 0.5f), -0.5f), 0.0f);
-  AxisTap t;
-  t.i0 = min((int)floorf(src), n - 1);
-  t.i1 = t.i0 + (t.i0 < n - 1 ? 1 : 0);
-  t.l1 = fminf(fmaxf(__fsub_rn(src, (float)t.i0), 0.0f), 1.0f);
-  t.l0 = __fsub_rn(1.0f, t.l1);
-  return t;
-}
 __global__ void terrain_upsample_kernel(const UpsampleParams p) {
   pdl_launch_dependents();
   pdl_wait();
@@ -172,20 +147,9 @@ __global__ void terrain_upsample_kernel(const UpsampleParams p) {
     ty = upsample_axis(p.oi + y, p.h, p.r);
     tx = upsample_axis(p.oj + x, p.w, p.r);
   }
-  float w00 = 0.f, w01 = 0.f, w10 = 0.f, w11 = 0.f;
-  if (p.small) {
-    w00 = __fmul_rn(ty.l0, tx.l0); w01 = __fmul_rn(ty.l0, tx.l1);
-    w10 = __fmul_rn(ty.l1, tx.l0); w11 = __fmul_rn(ty.l1, tx.l1);
-  }
-  const long r0 = (long)ty.i0 * p.w, r1 = (long)ty.i1 * p.w;
   auto sample = [&](const float* f) {
-    if (p.scale == 1) return f[r0 + tx.i0];
-    const float x00 = f[r0 + tx.i0], x01 = f[r0 + tx.i1], x10 = f[r1 + tx.i0], x11 = f[r1 + tx.i1];
-    if (p.small)
-      return __fmaf_rn(w11, x11, __fmaf_rn(w10, x10, __fmaf_rn(w00, x00, __fmul_rn(w01, x01))));
-    const float t0 = __fmaf_rn(tx.l0, x00, __fmul_rn(tx.l1, x01));
-    const float t1 = __fmaf_rn(tx.l0, x10, __fmul_rn(tx.l1, x11));
-    return __fmaf_rn(ty.l0, t0, __fmul_rn(ty.l1, t1));
+    if (p.scale == 1) return f[(long)ty.i0 * p.w + tx.i0];
+    return bilinear_at(f, p.w, ty, tx, p.small);
   };
   const long o = (long)y * p.W + x, plane_in = (long)p.h * p.w, plane_out = (long)p.H * p.W;
   const float e = sample(p.elev);

@@ -421,6 +421,40 @@ class WorldPipeline:
         body = postproc.upsample_crop(native["elev"], native["climate"], int(scale), oi, oj, H, W, payload=True)
         return postproc.to_host(body).numpy().tobytes(), (H, W)
 
+    def get_minecraft(self, i1: int, j1: int, i2: int, j2: int, scale: int = 1, noise: float = 1.0,
+                      noise_fn=None) -> dict:
+        """The Minecraft API's read-out (minecraft_api.py `_handle_1x` / `_handle_upsampled` up to the response):
+        {'elev', 'elev_smooth': fp32 [H, W], 'climate': fp32 [5, H, W] | None, 'biome': int16 [H, W]} over rows
+        [i1, i2) x columns [j1, j2) of the world upsampled `scale` times.  Scale 1 reads the window and, for the slope,
+        the window with a 1-pixel ring; scale >= 2 reads the native window padded by 2 pixels, upsamples it bit for bit
+        with the reference's torch CPU bilinear interpolation and, for noise > 0, adds the slope-scaled detail noise
+        to 'elev' ('elev_smooth' is without it).  'biome' holds the classifier's Minecraft biome ids; all plains when
+        there is no climate.  One launch on the device; CPU tensors (pinned copies) for WorldPipeline, CUDA tensors for
+        TerrainPipeline.
+
+        `noise_fn(cfg, i0, j0, h, w) -> fp32 [h, w]` supplies the FastNoiseLite noise planes (see inference/minecraft.py);
+        it must be a pure function of its arguments.  The default uses pyfastnoiselite and raises RuntimeError without it.
+        Raises ValueError for a non-integer window or scale, scale < 1, an empty window, more than 65535 rows or a
+        non-numeric `noise`.  The reference fails on a one-column window taller than one row (its Sobel `.squeeze()`
+        drops the column axis); here that window is classified like any other."""
+        from . import minecraft, postproc
+        (planes, biome), _ = minecraft.request(self._get_device, self.native_resolution, i1, j1, i2, j2, scale, noise,
+                                               noise_fn, payload=False)
+        if self._host_views:
+            planes, biome = postproc.to_host(planes), postproc.to_host(biome)
+        return {"elev": planes[0], "elev_smooth": planes[1], "climate": planes[2:] if planes.shape[0] == 7 else None,
+                "biome": biome}
+
+    def minecraft_payload(self, i1: int, j1: int, i2: int, j2: int, scale: int = 1, noise: float = 1.0,
+                          noise_fn=None) -> tuple:
+        """(body, (H, W)) of the Minecraft API's binary `GET /terrain`: body is `_binary_response(elev, biome=biome)`'s,
+        byte for byte -- int16-LE elevation (floor, clip; NaN packs as 0), then the int16-LE biome ids.  Packed on the
+        device and copied to the host once.  Arguments and errors as get_minecraft."""
+        from . import minecraft, postproc
+        body, hw = minecraft.request(self._get_device, self.native_resolution, i1, j1, i2, j2, scale, noise, noise_fn,
+                                     payload=True)
+        return postproc.to_host(body).numpy().tobytes(), hw
+
     def get_relief(self, i1: int, j1: int, i2: int, j2: int, **kw):
         """Shaded relief RGB [H, W, 3] of the elevation over pixel rows [i1,i2) x columns [j1,j2): `get_elev` and then
         `get_relief_map` on the device, with `resolution` defaulting to `native_resolution` as the explorer passes it
