@@ -15,7 +15,6 @@ tensor, which reads one 4-byte flag back after the launches.
 """
 from __future__ import annotations
 
-import ctypes as C
 import operator
 
 import numpy as np
@@ -25,10 +24,6 @@ from .. import _lib as L
 
 MAX_PIXELS = 1 << 24         # fp32 counts are exact integers up to here
 _FLAG_INF, _FLAG_RANGE, _FLAG_NOT_DOWNHILL = 1, 2, 4   # tdx.h TDX_FLOW_*
-
-
-def _p(t: torch.Tensor | None):
-    return C.c_void_p(None if t is None else t.data_ptr())
 
 
 def _shape(x) -> tuple:
@@ -88,18 +83,17 @@ def d8_flow(z, tol=1e-3):
         tol32 = float(np.float32(tol))
     zd = zz if on_device else _on_device(zz)
     h, w = zd.shape
-    with torch.cuda.device(zd.device):
-        kw = dict(device=zd.device)
-        kmax = torch.empty((h, w), dtype=torch.int8, **kw)
-        sink = torch.empty((h, w), dtype=torch.uint8, **kw)
-        rr = torch.empty((h, w), dtype=torch.int64, **kw)
-        cc = torch.empty((h, w), dtype=torch.int64, **kw)
-        flags = torch.empty(1, dtype=torch.int32, **kw)
-        L.check(L.lib().tdx_flow_d8(_p(zd), h, w, tol32, _p(kmax), _p(sink), _p(rr), _p(cc), _p(None), _p(None),
-                                    _p(flags), L.current_stream_ptr()))
-        if on_device:
-            _check_flags(flags, "d8_flow")
-            return rr, cc, sink.view(torch.bool), kmax.long()
+    kw = dict(device=zd.device)
+    kmax = torch.empty((h, w), dtype=torch.int8, **kw)
+    sink = torch.empty((h, w), dtype=torch.uint8, **kw)
+    rr = torch.empty((h, w), dtype=torch.int64, **kw)
+    cc = torch.empty((h, w), dtype=torch.int64, **kw)
+    flags = torch.empty(1, dtype=torch.int32, **kw)
+    L.call(L.lib().tdx_flow_d8, zd.device, zd.data_ptr(), h, w, tol32, kmax.data_ptr(), sink.data_ptr(), rr.data_ptr(),
+           cc.data_ptr(), None, None, flags.data_ptr())
+    if on_device:
+        _check_flags(flags, "d8_flow")
+        return rr, cc, sink.view(torch.bool), kmax.long()
     return rr.cpu().numpy(), cc.cpu().numpy(), sink.cpu().numpy().view(bool), kmax.cpu().numpy().astype(np.int64)
 
 
@@ -143,23 +137,23 @@ def flow_accumulation(z, rr, cc, is_sink):
     is_sink = _receiver_array(is_sink, "is_sink", shape, True)
     zd = zz if on_device else _on_device(zz)
     h, w = shape
-    with torch.cuda.device(zd.device):
-        rd, cd = _to_device(rr, zd.device, torch.int64), _to_device(cc, zd.device, torch.int64)
-        sd = _to_device(is_sink, zd.device, torch.uint8)
-        recv = torch.empty((h, w), dtype=torch.int32, device=zd.device)
-        indeg = torch.empty((h, w), dtype=torch.int32, device=zd.device)
-        flags = torch.empty(1, dtype=torch.int32, device=zd.device)
-        s = L.current_stream_ptr()
-        L.check(L.lib().tdx_flow_link(_p(zd), _p(rd), _p(cd), _p(sd), h, w, _p(recv), _p(indeg), _p(flags), s))
-        _check_flags(flags, "flow_accumulation")
-        a = _accumulate(zd, recv, indeg, s)
+    rd, cd = _to_device(rr, zd.device, torch.int64), _to_device(cc, zd.device, torch.int64)
+    sd = _to_device(is_sink, zd.device, torch.uint8)
+    recv = torch.empty((h, w), dtype=torch.int32, device=zd.device)
+    indeg = torch.empty((h, w), dtype=torch.int32, device=zd.device)
+    flags = torch.empty(1, dtype=torch.int32, device=zd.device)
+    L.call(L.lib().tdx_flow_link, zd.device, zd.data_ptr(), rd.data_ptr(), cd.data_ptr(), sd.data_ptr(), h, w,
+           recv.data_ptr(), indeg.data_ptr(), flags.data_ptr())
+    _check_flags(flags, "flow_accumulation")
+    a = _accumulate(zd, recv, indeg)
     return a if on_device else a.cpu().numpy()
 
 
-def _accumulate(zd, recv, indeg, stream) -> torch.Tensor:
+def _accumulate(zd, recv, indeg) -> torch.Tensor:
     state = torch.empty(zd.numel(), dtype=torch.int64, device=zd.device)
     a = torch.empty(zd.shape, dtype=torch.float32, device=zd.device)
-    L.check(L.lib().tdx_flow_accumulate(_p(zd), zd.numel(), _p(recv), _p(indeg), _p(state), _p(a), stream))
+    L.call(L.lib().tdx_flow_accumulate, zd.device, zd.data_ptr(), zd.numel(), recv.data_ptr(), indeg.data_ptr(),
+           state.data_ptr(), a.data_ptr())
     return a
 
 
@@ -176,17 +170,15 @@ def plot_flow_indicator(z, max_pool_kernel=1):
     k = max(k, 1)
     zd = zz if on_device else _on_device(zz)
     h, w = zd.shape
-    with torch.cuda.device(zd.device):
-        s = L.current_stream_ptr()
-        recv = torch.empty((h, w), dtype=torch.int32, device=zd.device)
-        indeg = torch.empty((h, w), dtype=torch.int32, device=zd.device)
-        flags = torch.empty(1, dtype=torch.int32, device=zd.device)
-        L.check(L.lib().tdx_flow_d8(_p(zd), h, w, float(np.float32(1e-3)), _p(None), _p(None), _p(None), _p(None),
-                                    _p(recv), _p(indeg), _p(flags), s))
-        a = _accumulate(zd, recv, indeg, s)
-        out = torch.empty((h // k, w // k), dtype=torch.float32, device=zd.device)
-        L.check(L.lib().tdx_flow_indicator(_p(a), h, w, k, _p(out), s))
-        if on_device:
-            _check_flags(flags, "plot_flow_indicator")
-            return out
+    recv = torch.empty((h, w), dtype=torch.int32, device=zd.device)
+    indeg = torch.empty((h, w), dtype=torch.int32, device=zd.device)
+    flags = torch.empty(1, dtype=torch.int32, device=zd.device)
+    L.call(L.lib().tdx_flow_d8, zd.device, zd.data_ptr(), h, w, float(np.float32(1e-3)), None, None, None, None,
+           recv.data_ptr(), indeg.data_ptr(), flags.data_ptr())
+    a = _accumulate(zd, recv, indeg)
+    out = torch.empty((h // k, w // k), dtype=torch.float32, device=zd.device)
+    L.call(L.lib().tdx_flow_indicator, zd.device, a.data_ptr(), h, w, k, out.data_ptr())
+    if on_device:
+        _check_flags(flags, "plot_flow_indicator")
+        return out
     return out.cpu().numpy()

@@ -94,39 +94,32 @@ def noise_planes(noise_fn, i1: int, j1: int, H: int, W: int, which, device) -> t
     return out
 
 
-@postproc._on_arg_device
 def readout(elev: torch.Tensor, climate, noise: torch.Tensor, scale: int, oi: int, oj: int, H: int, W: int,
             noise_scale: float, pixel_size_m: float, native_resolution: float, centre=None, payload: bool = False):
     """One `tdx_minecraft_readout` launch.  Returns (fp32 [7, H, W] = elev, elev_smooth, 5 climate planes (or [2, H, W]
     without climate), int16 biome [H, W]), or with `payload` the wire body as uint8 [4HW].  The scalars are the
     reference's Python doubles, each rounded to fp32 as torch rounds a Python scalar at every op."""
-    elev = postproc._chk(elev, "minecraft readout(elev)")
+    elev = postproc.check_plane(elev, "minecraft readout(elev)")
     h, w = elev.shape
     if centre is not None:
-        centre = postproc._chk(centre, "minecraft readout(centre)")
+        centre = postproc.check_plane(centre, "minecraft readout(centre)")
     if climate is not None:
-        ch, cw = (H, W) if scale == 1 else (h, w)
-        if not (isinstance(climate, torch.Tensor) and climate.is_cuda and climate.dtype == torch.float32
-                and tuple(climate.shape) == (5, ch, cw) and climate.device == elev.device):
-            raise L.TdxError(f"minecraft readout: climate must be a CUDA float32 [5, {ch}, {cw}] tensor on {elev.device}")
-        climate = climate.contiguous()
+        climate = postproc.check_plane(climate, "minecraft readout(climate)", (5, H, W) if scale == 1 else (5, h, w),
+                                       elev.device)
     noise = noise.contiguous()
     detail = int(scale > 1 and noise_scale > 0)
     scalars = (C.c_float(noise_scale * 100.0), C.c_float(noise_scale * 70.0), C.c_float(pixel_size_m),
                C.c_float(native_resolution), C.c_float(40.0 * pixel_size_m / 90.0))
-    ptr = lambda t: postproc._p(t) if t is not None else None
-    lib, s = L.lib(), L.current_stream_ptr()
-    head = (postproc._p(elev), h, w, scale, oi, oj, ptr(centre), ptr(climate), postproc._p(noise), H, W, detail,
-            *scalars)
+    head = (elev.data_ptr(), h, w, scale, oi, oj, None if centre is None else centre.data_ptr(),
+            None if climate is None else climate.data_ptr(), noise.data_ptr(), H, W, detail, *scalars)
     if payload:
         out = torch.empty((4 * H * W,), dtype=torch.uint8, device=elev.device)
-        L.check(lib.tdx_minecraft_readout(*head, None, None, None, None, postproc._p(out), s))
+        L.call(L.lib().tdx_minecraft_readout, elev.device, *head, None, None, None, None, out.data_ptr())
         return out
     planes = torch.empty((7 if climate is not None else 2, H, W), dtype=torch.float32, device=elev.device)
     biome = torch.empty((H, W), dtype=torch.int16, device=elev.device)
-    L.check(lib.tdx_minecraft_readout(*head, postproc._p(planes[0]), postproc._p(planes[1]),
-                                      postproc._p(planes[2]) if climate is not None else None, postproc._p(biome),
-                                      None, s))
+    L.call(L.lib().tdx_minecraft_readout, elev.device, *head, planes[0].data_ptr(), planes[1].data_ptr(),
+           planes[2].data_ptr() if climate is not None else None, biome.data_ptr(), None)
     return planes, biome
 
 

@@ -9,10 +9,6 @@ CUDA fp32 `[H, W]` and never leave the GPU.  There is no CPU path: CPU tensors r
 """
 from __future__ import annotations
 
-import ctypes as C
-
-import functools
-
 import numpy as np
 import torch
 
@@ -21,29 +17,17 @@ from .. import _lib as L
 LOWFREQ_MEAN, LOWFREQ_STD = -31.4, 38.6          # world_pipeline.py:1280-1281
 
 
-def _on_arg_device(fn):
-    """Run `fn` with the CUDA device of its first device-carrying argument (tensor or canvas) current: libtdx launches
-    on the current device and on its current stream (L.current_stream_ptr())."""
-    @functools.wraps(fn)
-    def wrapper(*a, **k):
-        for v in list(a) + list(k.values()):
-            dev = getattr(v, "device", None)
-            if isinstance(dev, torch.device) and dev.type == "cuda":
-                with torch.cuda.device(dev):
-                    return fn(*a, **k)
-        return fn(*a, **k)
-    return wrapper
-
-
-def _chk(x: torch.Tensor, name: str) -> torch.Tensor:
-    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 2):
-        raise L.TdxError(f"{name}: expected a CUDA float32 [H, W] tensor (the GPU read-out has no CPU path), got "
+def check_plane(x, name: str, shape=None, device=None) -> torch.Tensor:
+    """`x` made contiguous, after checking that it is a CUDA float32 tensor: [H, W] when `shape` is None, else exactly
+    `shape`, and on `device` when one is given.  Raises L.TdxError otherwise (the GPU read-out has no CPU path)."""
+    ok = isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32
+    ok = ok and (x.dim() == 2 if shape is None else tuple(x.shape) == tuple(shape))
+    if not (ok and (device is None or x.device == device)):
+        want = "[H, W]" if shape is None else list(shape)
+        on = "" if device is None else f" on {device}"
+        raise L.TdxError(f"{name}: expected a CUDA float32 {want} tensor{on} (the GPU read-out has no CPU path), got "
                          f"{getattr(x, 'device', None)} {getattr(x, 'dtype', None)} {tuple(getattr(x, 'shape', ()))}")
     return x.contiguous()
-
-
-def _p(t: torch.Tensor):
-    return C.c_void_p(t.data_ptr())
 
 
 def _resized_output_size(h: int, w: int, size) -> tuple[int, int]:
@@ -56,30 +40,27 @@ def _resized_output_size(h: int, w: int, size) -> tuple[int, int]:
     return new_h, new_w
 
 
-@_on_arg_device
 def resize_bilinear(x: torch.Tensor, size) -> torch.Tensor:
     """TF.resize(x, size, interpolation=BILINEAR) for an fp32 tensor (antialias on): width pass, then height pass."""
-    x = _chk(x, "resize_bilinear")
+    x = check_plane(x, "resize_bilinear")
     h, w = x.shape
     new_h, new_w = _resized_output_size(h, w, size)
-    s = L.current_stream_ptr()
     if new_w != w:
         y = torch.empty((h, new_w), dtype=torch.float32, device=x.device)
-        L.check(L.lib().tdx_resize_aa_axis(_p(x), h, w, _p(y), new_w, 1, s))
+        L.call(L.lib().tdx_resize_aa_axis, y.device, x.data_ptr(), h, w, y.data_ptr(), new_w, 1)
         x, w = y, new_w
     if new_h != h:
         y = torch.empty((new_h, w), dtype=torch.float32, device=x.device)
-        L.check(L.lib().tdx_resize_aa_axis(_p(x), h, w, _p(y), new_h, 0, s))
+        L.call(L.lib().tdx_resize_aa_axis, y.device, x.data_ptr(), h, w, y.data_ptr(), new_h, 0)
         x = y
     return x
 
 
-@_on_arg_device
 def pad_linear_extrapolation(x: torch.Tensor) -> torch.Tensor:
-    x = _chk(x, "pad_linear_extrapolation")
+    x = check_plane(x, "pad_linear_extrapolation")
     h, w = x.shape
     out = torch.empty((h + 2, w + 2), dtype=torch.float32, device=x.device)
-    L.check(L.lib().tdx_post_pad_extrapolate(_p(x), h, w, _p(out), L.current_stream_ptr()))
+    L.call(L.lib().tdx_post_pad_extrapolate, out.device, x.data_ptr(), h, w, out.data_ptr())
     return out
 
 
@@ -93,30 +74,28 @@ def resize_extrapolated(x: torch.Tensor, size) -> torch.Tensor:
     return out[ph:ph + th, pw:pw + tw]
 
 
-@_on_arg_device
 def gaussian_blur(x: torch.Tensor, kernel_size: int, sigma: float) -> torch.Tensor:
-    x = _chk(x, "gaussian_blur")
+    x = check_plane(x, "gaussian_blur")
     h, w = x.shape
     out = torch.empty_like(x)
-    L.check(L.lib().tdx_gaussian_blur(_p(x), h, w, _p(out), int(kernel_size), float(sigma), L.current_stream_ptr()))
+    L.call(L.lib().tdx_gaussian_blur, out.device, x.data_ptr(), h, w, out.data_ptr(), int(kernel_size), float(sigma))
     return out
 
 
-@_on_arg_device
 def _combine(a: torch.Tensor, b: torch.Tensor, signed_square: bool = False, int16: bool = False):
     """f(a + b) over two equally shaped (possibly strided-row) views."""
     assert a.shape == b.shape and a.stride(1) == 1 and b.stride(1) == 1
     h, w = a.shape
     out = torch.empty((h, w), dtype=torch.float32, device=a.device)
     out16 = torch.empty((h, w), dtype=torch.int16, device=a.device) if int16 else None
-    L.check(L.lib().tdx_post_combine(_p(a), a.stride(0), _p(b), b.stride(0), _p(out),
-                                     _p(out16) if int16 else None, h, w, int(signed_square), L.current_stream_ptr()))
+    L.call(L.lib().tdx_post_combine, out.device, a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), out.data_ptr(),
+           out16.data_ptr() if int16 else None, h, w, int(signed_square))
     return (out, out16) if int16 else out
 
 
 def laplacian_decode(residual: torch.Tensor, lowres: torch.Tensor, extrapolate: bool = False) -> torch.Tensor:
     """residual + upsampled lowres (laplacian_encoder.py:95-131, pre_padded=False)."""
-    residual = _chk(residual, "laplacian_decode")
+    residual = check_plane(residual, "laplacian_decode")
     up = resize_extrapolated(lowres, residual.shape) if extrapolate else resize_bilinear(lowres, tuple(residual.shape))
     return _combine(residual, up)
 
@@ -143,7 +122,6 @@ def padded_window(i1: int, j1: int, i2: int, j2: int, scale: int, sigma: float =
     return pi1, pj1, pi2, pj2
 
 
-@_on_arg_device
 def compute_elev(residual_canvas, latents_canvas, i1: int, j1: int, i2: int, j2: int, scale: int, residual_mean: float,
                  residual_std: float, sigma: float = 5, as_int16: bool = False):
     """Elevation in metres over pixel rows [i1, i2) x columns [j1, j2) (world_pipeline.py:1277-1313).
@@ -162,12 +140,12 @@ def compute_elev(residual_canvas, latents_canvas, i1: int, j1: int, i2: int, j2:
     r, lat = r.float().contiguous(), lat.float().contiguous()
     hp, wp = r.shape[-2:]
     hl, wl = lat.shape[-2:]
-    s = L.current_stream_ptr()
     residual_p = torch.empty((hp, wp), dtype=torch.float32, device=r.device)
     lowfreq_p = torch.empty((hl, wl), dtype=torch.float32, device=r.device)
-    L.check(L.lib().tdx_post_normalize(_p(r[0]), _p(r[1]), wp, _p(residual_p), hp, wp, float(residual_std),
-                                       float(residual_mean), s))
-    L.check(L.lib().tdx_post_normalize(_p(lat[4]), _p(lat[-1]), wl, _p(lowfreq_p), hl, wl, LOWFREQ_STD, LOWFREQ_MEAN, s))
+    L.call(L.lib().tdx_post_normalize, r.device, r[0].data_ptr(), r[1].data_ptr(), wp, residual_p.data_ptr(), hp, wp,
+           float(residual_std), float(residual_mean))
+    L.call(L.lib().tdx_post_normalize, r.device, lat[4].data_ptr(), lat[-1].data_ptr(), wl, lowfreq_p.data_ptr(), hl,
+           wl, LOWFREQ_STD, LOWFREQ_MEAN)
     residual_p, lowfreq_p = laplacian_denoise(residual_p, lowfreq_p, sigma)
     up = resize_bilinear(lowfreq_p, (hp, wp))
     oi, oj = i1 - pi1, j1 - pj1
@@ -200,7 +178,6 @@ def terrain_window(i1: int, j1: int, i2: int, j2: int, scale: int):
     return ni1 - 1, nj1 - 1, ni2 + 1, nj2 + 1, scale + (i1 - ni1 * scale), scale + (j1 - nj1 * scale)
 
 
-@_on_arg_device
 def upsample_crop(elev: torch.Tensor, climate: torch.Tensor | None, scale: int, oi: int, oj: int, H: int, W: int,
                   payload: bool = False) -> torch.Tensor:
     """The terrain API's upsample + crop (api.py:139-164, torch's CPU F.interpolate(scale_factor=scale, mode='bilinear',
@@ -208,42 +185,38 @@ def upsample_crop(elev: torch.Tensor, climate: torch.Tensor | None, scale: int, 
     [oi, oi+H) x [oj, oj+W) of the upsampled window only; scale == 1 is the plain crop.  Returns one CUDA tensor: fp32
     [6, H, W] (elevation, then the 5 climate planes) or [1, H, W] without climate; with `payload`, the wire body of
     api.py:80-100 as uint8 [2HW (+ 16HW with climate)]."""
-    elev = _chk(elev, "upsample_crop(elev)")
+    elev = check_plane(elev, "upsample_crop(elev)")
     h, w = elev.shape
     if climate is not None:
-        if not (isinstance(climate, torch.Tensor) and climate.is_cuda and climate.dtype == torch.float32
-                and tuple(climate.shape) == (5, h, w) and climate.device == elev.device):
-            raise L.TdxError(f"upsample_crop: climate must be a CUDA float32 [5, {h}, {w}] tensor on {elev.device}")
-        climate = climate.contiguous()
-    s = L.current_stream_ptr()
-    clim_p = _p(climate) if climate is not None else None
+        climate = check_plane(climate, "upsample_crop(climate)", (5, h, w), elev.device)
+    clim_p = climate.data_ptr() if climate is not None else None
     if payload:
         out = torch.empty((H * W * (18 if climate is not None else 2),), dtype=torch.uint8, device=elev.device)
-        L.check(L.lib().tdx_terrain_upsample(_p(elev), clim_p, h, w, scale, oi, oj, H, W, None, None, _p(out), s))
+        L.call(L.lib().tdx_terrain_upsample, elev.device, elev.data_ptr(), clim_p, h, w, scale, oi, oj, H, W, None,
+               None, out.data_ptr())
         return out
     out = torch.empty((6 if climate is not None else 1, H, W), dtype=torch.float32, device=elev.device)
-    L.check(L.lib().tdx_terrain_upsample(_p(elev), clim_p, h, w, scale, oi, oj, H, W, _p(out[0]),
-                                         _p(out[1]) if climate is not None else None, None, s))
+    L.call(L.lib().tdx_terrain_upsample, elev.device, elev.data_ptr(), clim_p, h, w, scale, oi, oj, H, W,
+           out[0].data_ptr(), out[1].data_ptr() if climate is not None else None, None)
     return out
 
 
-@_on_arg_device
 def to_host(t: torch.Tensor) -> torch.Tensor:
-    """One device -> host copy into pinned memory (torch's caching host allocator), on the current stream, waited for."""
+    """One device -> host copy into pinned memory (torch's caching host allocator), on the current stream of `t`'s
+    device, waited for."""
     staging = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
     staging.copy_(t, non_blocking=True)
     torch.cuda.current_stream(t.device).synchronize()
     return staging
 
 
-@_on_arg_device
 def compute_climate(coarse_canvas, i1: int, j1: int, i2: int, j2: int, elev: torch.Tensor, scale: int) -> torch.Tensor:
     """Climate over pixel rows [i1, i2) x columns [j1, j2) (WorldPipeline._compute_climate, world_pipeline.py:1314-1365):
     fp32 CUDA [5, H, W] = {temperature with the local lapse-rate correction, coarse channels 3, 4, 5, lapse rate}.
 
     `coarse_canvas[:, a:b, c:d]` returns the un-normalised planes of the coarse canvas (one cell = 32*scale pixels; channel
     0 = signed-sqrt elevation, 2 = temperature, last = weight); `elev` is compute_elev's result for the same window."""
-    elev = _chk(elev, "compute_climate(elev)")
+    elev = check_plane(elev, "compute_climate(elev)")
     if tuple(elev.shape) != (i2 - i1, j2 - j1):
         raise ValueError(f"elev is {tuple(elev.shape)}, the window is {(i2 - i1, j2 - j1)}")
     S = 32 * scale
@@ -256,18 +229,18 @@ def compute_climate(coarse_canvas, i1: int, j1: int, i2: int, j2: int, elev: tor
         raise L.TdxError("compute_climate: the coarse canvas must return CUDA tensors (no CPU path)")
     c = c.float().contiguous()
     nch, hc, wc = c.shape[0] - 1, c.shape[1], c.shape[2]
-    s = L.current_stream_ptr()
     cmap = torch.empty((nch, hc, wc), dtype=torch.float32, device=c.device)
     for k in range(nch):                               # coarse_map = coarse_init[:-1] / coarse_init[-1:]
-        L.check(L.lib().tdx_post_normalize(_p(c[k]), _p(c[-1]), wc, _p(cmap[k]), hc, wc, 1.0, 0.0, s))
+        L.call(L.lib().tdx_post_normalize, c.device, c[k].data_ptr(), c[-1].data_ptr(), wc, cmap[k].data_ptr(), hc,
+               wc, 1.0, 0.0)
     hs, ws = hc - win + 1, wc - win + 1
     t_sea = torch.empty((hs, ws), dtype=torch.float32, device=c.device)
     beta = torch.empty((hs, ws), dtype=torch.float32, device=c.device)
     # local_baseline_temperature_torch(coarse_map[2], coarse_elev_denorm, win=15, fallback_threshold=0.02), defaults of
     # inference/postprocessing.py:262-270 otherwise
-    L.check(L.lib().tdx_lapse_rate(_p(cmap[2]), _p(cmap[0]), hc, wc, win, -0.012, 0.0, -0.0065, 1e-6, 0.02, _p(t_sea),
-                                   _p(beta), s))
+    L.call(L.lib().tdx_lapse_rate, c.device, cmap[2].data_ptr(), cmap[0].data_ptr(), hc, wc, win, -0.012, 0.0,
+           -0.0065, 1e-6, 0.02, t_sea.data_ptr(), beta.data_ptr())
     out = torch.empty((5, i2 - i1, j2 - j1), dtype=torch.float32, device=c.device)
-    L.check(L.lib().tdx_climate_sample(_p(t_sea), _p(beta), _p(cmap), nch, hc, wc, win // 2, _p(elev), i1, j1, i2 - i1,
-                                       j2 - j1, S, ci1, cj1, _p(out), s))
+    L.call(L.lib().tdx_climate_sample, c.device, t_sea.data_ptr(), beta.data_ptr(), cmap.data_ptr(), nch, hc, wc,
+           win // 2, elev.data_ptr(), i1, j1, i2 - i1, j2 - j1, S, ci1, cj1, out.data_ptr())
     return out

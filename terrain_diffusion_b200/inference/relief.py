@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 from .. import _lib as L
+from .postproc import check_plane
 
 # matplotlib's `terrain` colormap (matplotlib/_cm.py `_terrain_data`): six (position, RGB) stops, linearly interpolated
 TERRAIN_STOPS = ((0.00, (0.2, 0.2, 0.6)), (0.15, (0.0, 0.6, 1.0)), (0.25, (0.0, 0.8, 0.4)),
@@ -71,31 +72,23 @@ def _lut_on(device: torch.device) -> torch.Tensor:
     return _luts[device]
 
 
-def _p(t: torch.Tensor):
-    return C.c_void_p(t.data_ptr())
-
-
 def gaussian_filter(x: torch.Tensor, sigmas, *, nan_fill: float | None = None) -> torch.Tensor:
     """scipy.ndimage.gaussian_filter(x, sigma) (mode 'reflect', truncate 4, fp32 between the axes), bit for bit, for one
     or two sigmas in one pair of launches: CUDA fp32 [H, W] -> [len(sigmas), H, W].  With nan_fill, NaN is read as it."""
-    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 2):
-        raise L.TdxError("gaussian_filter: expected a CUDA float32 [H, W] tensor")
+    x = check_plane(x, "gaussian_filter")
     sigmas = [float(s) for s in sigmas]
     taps = [gaussian_taps(s) for s in sigmas]
     radius = [len(t) // 2 for t in taps]
     if not 1 <= len(sigmas) <= 2 or max(radius) > MAX_RADIUS:
         raise ValueError(f"gaussian_filter: 1 or 2 sigmas with int(4 sigma + 0.5) <= {MAX_RADIUS}, got {sigmas}")
-    x = x.contiguous()
     h, w = x.shape
     w64 = np.ascontiguousarray(np.concatenate(taps), dtype=np.float64)
     r32 = (C.c_int32 * len(radius))(*radius)
-    with torch.cuda.device(x.device):
-        tmp = torch.empty((len(sigmas), h, w), dtype=torch.float32, device=x.device)
-        out = torch.empty_like(tmp)
-        L.check(L.lib().tdx_relief_gaussian(_p(x), h, w, int(nan_fill is not None),
-                                            0.0 if nan_fill is None else float(nan_fill), len(sigmas),
-                                            w64.ctypes.data_as(C.POINTER(C.c_double)), r32, _p(tmp), _p(out),
-                                            L.current_stream_ptr()))
+    tmp = torch.empty((len(sigmas), h, w), dtype=torch.float32, device=x.device)
+    out = torch.empty_like(tmp)
+    L.call(L.lib().tdx_relief_gaussian, x.device, x.data_ptr(), h, w, int(nan_fill is not None),
+           0.0 if nan_fill is None else float(nan_fill), len(sigmas), w64.ctypes.data_as(C.POINTER(C.c_double)), r32,
+           tmp.data_ptr(), out.data_ptr())
     return out
 
 
@@ -136,17 +129,15 @@ def get_relief_map(elevation, climate, biome, flow, *, azimuths=(315.0, 45.0, 13
     else:
         host = elevation.detach().cpu().numpy() if isinstance(elevation, torch.Tensor) else np.asarray(elevation)
         elev = torch.from_numpy(np.ascontiguousarray(host, dtype=np.float32)).cuda()
-    with torch.cuda.device(elev.device):
-        out = _relief(elev.contiguous(), azimuths, sigma_large, sigma_small, resolution, relief, vmin, vmax)
+    out = _relief(elev.contiguous(), azimuths, sigma_large, sigma_small, resolution, relief, vmin, vmax)
     return out if on_device else out.cpu().numpy()
 
 
 def _relief(elev, azimuths, sigma_large, sigma_small, resolution, relief, vmin, vmax):
     h, w = elev.shape
     dev = elev.device
-    s = L.current_stream_ptr()
     stats = torch.empty(3, dtype=torch.int32, device=dev)
-    L.check(L.lib().tdx_relief_stats(_p(elev), h * w, _p(stats), s))
+    L.call(L.lib().tdx_relief_stats, dev, elev.data_ptr(), h * w, stats.data_ptr())
     has_nan = int(stats[0]) > 0
     fill = nanmedian_fill(elev) if has_nan else 0.0
     blurred = gaussian_filter(elev, (sigma_large, sigma_small), nan_fill=fill if has_nan else None)
@@ -156,8 +147,8 @@ def _relief(elev, azimuths, sigma_large, sigma_small, resolution, relief, vmin, 
     user_range = vmin is not None and vmax is not None
     lo, hi = (max(0.0, float(vmin)), float(vmax)) if user_range else (0.0, 1.0)
     out = torch.empty((h, w, 3), dtype=torch.float32, device=dev)
-    L.check(L.lib().tdx_relief_shade(_p(elev), _p(blurred), _p(stats), _p(_lut_on(dev)), h, w, int(has_nan), fill,
-                                     15 * resolution / 90, float(np.deg2rad(az_deg)), float(np.sin(alt)),
-                                     float(np.cos(alt)), float(relief), 1 - relief, int(user_range), lo,
-                                     hi - lo + 1e-8, int(lo == 0.0), _p(out), s))
+    L.call(L.lib().tdx_relief_shade, dev, elev.data_ptr(), blurred.data_ptr(), stats.data_ptr(),
+           _lut_on(dev).data_ptr(), h, w, int(has_nan), fill, 15 * resolution / 90, float(np.deg2rad(az_deg)),
+           float(np.sin(alt)), float(np.cos(alt)), float(relief), 1 - relief, int(user_range), lo, hi - lo + 1e-8,
+           int(lo == 0.0), out.data_ptr())
     return out
