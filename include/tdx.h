@@ -222,6 +222,14 @@ int tdx_pack_weighted(float* out, const float* x, const float* w, int32_t n_img,
  * window + F.interpolate(mode='nearest') (world_pipeline.py:1223-1226). */
 int tdx_window_to_cond(float* out, const float* packed, int32_t n_img, int32_t packed_channels, int32_t keep, int32_t h,
                        int32_t w, int32_t factor, void* stream);
+/* Coarse-tile epilogue (world_pipeline.py:948-958) in one launch: x [n_img][6][size][size] raw solve output ->
+ * out [n_img][7][size/pool][size/pool] = cat([v w, w]), v = pool(x / sigma_data * stds + means with channel 1 replaced
+ * by ch0 - ch1) bit for bit with the reference's fp32 CPU ops.  Channel 0 pools by elev_mode, channel 1 by p5_mode
+ * (0 avg, 1 max, 2 min), channels 2-5 by avg; pool == 1 does not pool.  size <= 64.  means / stds: 6 floats on the
+ * device; w: the [size/pool]^2 blend weights. */
+int tdx_coarse_epilogue(float* out, const float* x, const float* means, const float* stds, const float* w,
+                        int32_t n_img, int32_t size, int32_t pool, int32_t elev_mode, int32_t p5_mode, float sigma_data,
+                        void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Elevation read-out (WorldPipeline._compute_elev, inference/world_pipeline.py:1277-1313): the reference normalises

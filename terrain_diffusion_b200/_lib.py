@@ -126,6 +126,9 @@ def _declare(l: C.CDLL) -> None:
     l.tdx_window_to_cond.restype = C.c_int
     l.tdx_window_to_cond.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                      C.c_int32, C.c_void_p]
+    l.tdx_coarse_epilogue.restype = C.c_int
+    l.tdx_coarse_epilogue.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                      C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_void_p]
     l.tdx_post_normalize.restype = C.c_int
     l.tdx_post_normalize.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32, C.c_float,
                                      C.c_float, C.c_void_p]

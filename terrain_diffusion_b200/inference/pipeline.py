@@ -16,11 +16,18 @@ the coarse stage (`synthetic_map.py`, Perlin noise + WorldClim rasters).  Pass `
 store) is not implemented -- the window cache is the byte-limited HBM LRU of `LazyCanvas` (`cache_limit`, like the
 reference's MemoryTileStore).  `torch_compile` is accepted and ignored: every U-Net evaluation already is one CUDA
 graph of hand-written kernels.
+
+`coarse_pooling = p` (1, 2, 4, 8 or 16; world_pipeline.py:909-1016) pools every finished coarse solve by p on the
+device, channel 0 by `elev_coarse_pool_mode` and channel 1 by `p5_coarse_pool_mode` ('max', 'min', anything else
+averages), channels 2-5 by average, so the coarse canvas has p times fewer cells per axis (windows of (64/p)^2 at a
+stride of 48/p) and the latent stage and the climate read-out see coarser terrain.  The windows' conditioning cells and
+noise do not change.  Any other value raises ValueError in the constructor (the reference asserts only in `bind()`).
 """
 from __future__ import annotations
 
 import json
 import math
+import operator
 from pathlib import Path
 
 import numpy as np
@@ -28,7 +35,7 @@ import torch
 
 from ..scheduler import EDMDPMSolverMultistepScheduler
 from .lazy_canvas import LazyCanvas, TensorWindow
-from .stages import coarse_stage_tile, decoder_stage_tile, latent_stage_tiles
+from .stages import coarse_geometry, coarse_stage_tile, decoder_stage_tile, latent_stage_tiles
 from .tiling import linear_weight_window
 
 # seed offsets of the latent stage's noise fields: _build_latent_stage (world_pipeline.py:1133-1203) passes 5819 to the
@@ -75,8 +82,8 @@ class WorldPipeline:
         from .noise import next_seed
         if T not in (1, 2):
             raise ValueError(f"T must be 1 or 2, got {T}")
-        if coarse_pooling != 1:
-            raise NotImplementedError("coarse_pooling > 1 is host-side pooling of finished coarse tiles; not on the GPU path")
+        coarse_geometry(coarse_pooling)                  # ValueError unless it divides 64 and 48 (world_pipeline.py:969-970)
+        coarse_pooling = operator.index(coarse_pooling)
         self.T = T
         self.seed = (int(seed) & 0xFFFFFFFFFFFFFFFF) if seed is not None else next_seed(None)
         sizes = [latents_batch_size] if isinstance(latents_batch_size, int) else sorted(latents_batch_size)
@@ -280,16 +287,23 @@ class WorldPipeline:
         hist = torch.as_tensor(self.kwargs["histogram_raw"], dtype=torch.float32).view(1, -1)
         ww64 = linear_weight_window(64, dev)
 
-        # ---- coarse: 64^2 tiles, stride 48, 20-step DPM-Solver++
+        # ---- coarse: 64^2 solves at stride 48, 20-step DPM-Solver++, each pooled by coarse_pooling = p into a
+        # (64/p)^2 window at stride 48/p of the coarse canvas
         coarse_sched = EDMDPMSolverMultistepScheduler(sigma_min=0.002, sigma_max=80, sigma_data=0.5)
+        pool = self.kwargs["coarse_pooling"]
+        c_tile, c_stride = coarse_geometry(pool)
+        ww_coarse = linear_weight_window(c_tile, dev)
 
         def f_coarse(ctx):
             _, i, j = ctx
             smap = self._conditioning_model_input(i * 48, i * 48 + 64, j * 48, j * 48 + 64)
             return coarse_stage_tile(self.coarse_model, coarse_sched, self.seed, ctx, smap, self._t_cond,
-                                     self._cond_inputs, ww64, self.kwargs["coarse_means"], self.kwargs["coarse_stds"])
+                                     self._cond_inputs, ww_coarse, self.kwargs["coarse_means"],
+                                     self.kwargs["coarse_stds"], 20, pool, self.kwargs["elev_coarse_pool_mode"],
+                                     self.kwargs["p5_coarse_pool_mode"])
 
-        coarse = self._canvas("coarse", 7, f_coarse, TensorWindow((7, 64, 64), (7, 48, 48)), dev, cache_limit=lim)
+        coarse = self._canvas("coarse", 7, f_coarse, TensorWindow((7, c_tile, c_tile), (7, c_stride, c_stride)), dev,
+                              cache_limit=lim)
 
         # ---- latents: 64^2 tiles, stride 32; T=2: two consistency phases with a blend in between, T=1: both phases per
         # tile; batches padded to the legal sizes so that only a handful of plans exist
@@ -478,10 +492,12 @@ class TerrainPipeline(WorldPipeline):
                  cond_snr, histogram_raw, latents_means, latents_stds, latents_batch_size: int = 16,
                  decoder_tile_size: int = 512, decoder_tile_stride: int = 384, latent_compression: int = 8,
                  t_inter: float | None = None, residual_mean: float | None = None, residual_std: float | None = None,
-                 native_resolution: float = 90.0, cache_limit: int | None = None):
+                 native_resolution: float = 90.0, cache_limit: int | None = None, coarse_pooling: int = 1,
+                 elev_coarse_pool_mode: str = "avg", p5_coarse_pool_mode: str = "avg"):
         super().__init__(seed=seed, latents_batch_size=latents_batch_size, native_resolution=native_resolution,
                          latent_compression=latent_compression, cond_snr=[float(v) for v in cond_snr],
-                         residual_mean=residual_mean, residual_std=residual_std,
+                         coarse_pooling=coarse_pooling, elev_coarse_pool_mode=elev_coarse_pool_mode,
+                         p5_coarse_pool_mode=p5_coarse_pool_mode, residual_mean=residual_mean, residual_std=residual_std,
                          coarse_means=[float(v) for v in coarse_means], coarse_stds=[float(v) for v in coarse_stds],
                          cache_limit=cache_limit, decoder_tile_size=decoder_tile_size,
                          decoder_tile_stride=decoder_tile_stride, conditioning_fn=conditioning_fn,

@@ -12,7 +12,8 @@ around the U-Net, `.item()`, D2H -- is organised here around ONE fused program p
                        (tdx_pack_weighted); normalise-on-read + nearest upsampling of the latent window one launch
                        (tdx_window_to_cond).
   coarse stage         `get_diffusion_solve`: the 20-step DPM-Solver++ solve as one graph, the embeddings of all steps
-                       from one batched call.
+                       from one batched call.  De-normalisation, the channel-1 difference, `coarse_pooling` and the
+                       packed output are one launch (tdx_coarse_epilogue).
 
 Noise comes from the bit-compatible GPU generator (same seeds as the reference), nothing synchronises with the host and
 nothing leaves the GPU.  Taken as arguments, because the reference computes them outside the hot path: the synthetic
@@ -21,6 +22,7 @@ conditioning map of the coarse stage and the blended dependency windows the canv
 from __future__ import annotations
 
 import math
+import operator
 
 import torch
 
@@ -185,18 +187,66 @@ def latent_stage_tiles(model, seed: int, ctxs, samples, cond_imgs, t: float, wei
 
 
 # ------------------------------------------------------------------------------------------------ coarse stage
+COARSE_POOL_SIZES = tuple(n for n in range(1, COARSE_TILE + 1) if COARSE_TILE % n == 0 and COARSE_STRIDE % n == 0)
+_POOL_MODE_FLAGS = {"max": 1, "min": 2}       # tdx_coarse_epilogue's flags; any other mode averages (:994-1002)
+
+
+def coarse_geometry(pool_size) -> tuple:
+    """(tile, stride) of the coarse canvas in pooled cells for `coarse_pooling = pool_size` (world_pipeline.py:961-992):
+    window (0, i, j) is still the 64^2 solve at conditioning cells (48 i, 48 j), pooled to tile^2 cells, blended with
+    `linear_weight_window(tile)` at a stride of 48 / pool_size.  Raises ValueError unless pool_size is an integer that
+    divides both 64 and 48, i.e. one of COARSE_POOL_SIZES."""
+    try:
+        n = operator.index(pool_size)
+    except TypeError:
+        n = None
+    if n not in COARSE_POOL_SIZES:
+        raise ValueError(f"coarse_pooling must be an integer dividing both the coarse tile ({COARSE_TILE}) and its "
+                         f"stride ({COARSE_STRIDE}), one of {list(COARSE_POOL_SIZES)}; got {pool_size!r}")
+    return COARSE_TILE // n, COARSE_STRIDE // n
+
+
+def pool_mode_flag(mode) -> int:
+    """The reference's `_pool_channel` mode string as tdx_coarse_epilogue's flag: 'max' 1, 'min' 2, anything else avg 0."""
+    return _POOL_MODE_FLAGS.get(mode, 0) if isinstance(mode, str) else 0
+
+
+def coarse_epilogue(sample: torch.Tensor, means: torch.Tensor, stds: torch.Tensor, window: torch.Tensor,
+                    pool_size: int = 1, elev_pool_mode: str = "avg", p5_pool_mode: str = "avg",
+                    sigma_data: float = 0.5) -> torch.Tensor:
+    """[n, 6, 64, 64] raw solve output -> [n, 7, 64/p, 64/p] packed coarse tiles in one launch (world_pipeline.py:948-958):
+    de-normalise (x / sigma_data * stds + means), channel 1 = ch0 - ch1, pool by p (channel 0 by elev_pool_mode, 1 by
+    p5_pool_mode, 2-5 avg; p = 1 does not pool), cat([v w, w]); bit for bit with the reference's fp32 CPU ops.
+    means / stds: 6 fp32 values and window: the [64/p, 64/p] blend weights, all on sample's device."""
+    tile, _ = coarse_geometry(pool_size)
+    n, c, h, w = sample.shape
+    if (c, h, w) != (6, COARSE_TILE, COARSE_TILE) or sample.dtype != torch.float32 or not sample.is_contiguous():
+        raise ValueError(f"coarse_epilogue: sample must be a contiguous fp32 [n, 6, 64, 64] tensor, got "
+                         f"{sample.dtype} {tuple(sample.shape)}")
+    for name, t, shape in (("means", means, (6,)), ("stds", stds, (6,)), ("window", window, (tile, tile))):
+        if tuple(t.shape) != shape or t.dtype != torch.float32 or not t.is_contiguous() or t.device != sample.device:
+            raise ValueError(f"coarse_epilogue: {name} must be a contiguous fp32 {list(shape)} tensor on "
+                             f"{sample.device}, got {t.dtype} {tuple(t.shape)} on {t.device}")
+    out = torch.empty((n, 7, tile, tile), dtype=torch.float32, device=sample.device)
+    L.call(L.lib().tdx_coarse_epilogue, sample.device, out.data_ptr(), sample.data_ptr(), means.data_ptr(),
+           stds.data_ptr(), window.data_ptr(), n, COARSE_TILE, operator.index(pool_size), pool_mode_flag(elev_pool_mode),
+           pool_mode_flag(p5_pool_mode), float(sigma_data))
+    return out
+
+
 @torch.no_grad()
 def coarse_stage_tile(model, scheduler, seed: int, ctx, synthetic_map: torch.Tensor, t_cond: torch.Tensor,
                       cond_inputs, weight_window: torch.Tensor, coarse_means, coarse_stds, num_steps: int = 20,
-                      pool_size: int = 1) -> torch.Tensor:
+                      pool_size: int = 1, elev_pool_mode: str = "avg", p5_pool_mode: str = "avg") -> torch.Tensor:
     """Coarse window (0, i, j): 20-step DPM-Solver++ solve conditioned on the noised synthetic map
-    (world_pipeline.py:909-959).  synthetic_map: the raw [5, 64, 64] conditioning of this window (built by the
-    reference's Perlin / WorldClim machinery, out of scope).  Returns the packed [7, 64, 64] tile."""
-    if pool_size != 1:
-        raise NotImplementedError("coarse_pooling > 1 is host-side pooling of the finished tile; not on the GPU path")
+    (world_pipeline.py:909-959).  synthetic_map: the raw [5, 64, 64] conditioning of conditioning cells
+    (48 i .. 48 i + 64, 48 j .. 48 j + 64) whatever the pooling (built by the reference's Perlin / WorldClim machinery,
+    out of scope).  Returns the packed [7, 64/p, 64/p] tile, p = pool_size (see coarse_geometry / coarse_epilogue);
+    weight_window is the [64/p, 64/p] blend window."""
+    coarse_geometry(pool_size)                                   # argument errors before any device work
     dev = model.device
     T = COARSE_TILE
-    y0, x0 = ctx[1] * COARSE_STRIDE, ctx[2] * COARSE_STRIDE
+    y0, x0 = ctx[1] * COARSE_STRIDE, ctx[2] * COARSE_STRIDE      # = i * (48 // p) * p: p divides 48 (:919-920)
     means = _const_on(dev, torch.as_tensor(coarse_means, dtype=torch.float32))
     stds = _const_on(dev, torch.as_tensor(coarse_stds, dtype=torch.float32))
     sel = [0, 2, 3, 4, 5]                                        # model statistics of the map's five channels (:925)
@@ -207,6 +257,5 @@ def coarse_stage_tile(model, scheduler, seed: int, ctx, synthetic_map: torch.Ten
     noise = gaussian_noise_patch(seed + 1, y0, x0, T, T, 6, T, T, device=dev)[None]
     sample = solve.run(noise * float(scheduler.sigmas[0]), cond,
                        conditional_inputs=[_const_on(dev, c) for c in cond_inputs])
-    out = sample / float(scheduler.config.sigma_data) * stds.view(1, -1, 1, 1) + means.view(1, -1, 1, 1)
-    out[:, 1] = out[:, 0] - out[:, 1]                            # channel 1 is predicted as (ch0 - ch1) (:953)
-    return pack_weighted(out.contiguous(), _f32(weight_window, dev))[0]
+    return coarse_epilogue(sample.contiguous(), means, stds, _f32(weight_window, dev), pool_size, elev_pool_mode,
+                           p5_pool_mode, float(scheduler.config.sigma_data))[0]
