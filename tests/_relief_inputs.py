@@ -13,6 +13,13 @@ def _nan_case():
     return e
 
 
+def _inf_case():
+    e = field(48, 32, 40, 400.0, 300.0)
+    e[4, 5] = np.inf
+    e[26, 33] = -np.inf
+    return e
+
+
 CASES = {
     # name: (elevation builder, get_relief_map keyword arguments)
     "mixed": (lambda: field(41, 256, 320, 300.0, 600.0), {}),                               # land + ocean, vmin == 0
@@ -23,6 +30,13 @@ CASES = {
     "vrange": (lambda: field(46, 96, 128, 500.0, 400.0),
                {"vmin": 300.0, "vmax": 1800.5, "azimuths": (45.0,), "sigma_large": 3, "sigma_small": 0.8}),
     "ocean": (lambda: field(47, 80, 72, -3000.0, 400.0), {}),
+    # branches the cases above do not reach
+    "inf": (_inf_case, {"sigma_large": 1.5, "sigma_small": 0.5}),        # +-inf: fallback range, NaN around +inf
+    "relief2": (lambda: field(49, 24, 32, 300.0, 900.0), {"relief": 2.0}),  # gain < 0 on dark slopes, clipped to 0
+    "vmin_only": (lambda: field(50, 24, 32, 300.0, 600.0), {"vmin": 500.0}),  # one bound alone: the data's range
+    "vmax_only": (lambda: field(51, 24, 32, 300.0, 600.0), {"vmax": 700.0}),
+    "vmin_above": (lambda: field(52, 24, 32, 400.0, 300.0), {"vmin": 5000.0, "vmax": 9000.0}),  # land is black
+    "abyss": (lambda: field(54, 24, 32, -8000.0, 3000.0), {}),                # below -10000 m: the depth clip
 }
 
 
@@ -40,3 +54,14 @@ def relief_case(name):
     """(elevation fp32 [H, W], keyword arguments) of one case."""
     build, kw = CASES[name]
     return build(), dict(kw)
+
+
+def bench_field(n: int) -> np.ndarray:
+    """The elevation tools/bench_relief.py renders at n x n (a copy of its seeded builder): a smooth field with land
+    and ocean."""
+    rng = np.random.RandomState(n)
+    y, x = np.mgrid[0:n, 0:n].astype(np.float64) / n
+    e = np.zeros((n, n))
+    for _ in range(6):
+        e += rng.uniform(300, 900) * np.sin(rng.uniform(2, 20) * y + rng.uniform(2, 20) * x + rng.uniform(0, 6.28))
+    return (e + 200 + 30 * rng.randn(n, n)).astype(np.float32)

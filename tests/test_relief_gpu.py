@@ -23,12 +23,12 @@ from terrain_diffusion_b200.inference import TerrainPipeline, get_relief_map
 from terrain_diffusion_b200.inference import relief as R
 from terrain_diffusion_b200.models import EDMUnet2D
 from tests._post_inputs import field
+from tests._relief_contract import TOL, compare
 from tests._relief_inputs import CASES, golden_stride, relief_case
 from tests.test_oracle_golden import BASE_CFG, COARSE_CFG
 
 pytestmark = pytest.mark.gpu
 G = np.load(Path(__file__).resolve().parent / "golden" / "relief_golden.npz")
-TOL, BOUNDARY = 2e-5, 1e-4
 
 
 @pytest.mark.parametrize("shape", [(2, 2), (5, 7), (33, 17), (129, 65), (1024, 1024)])
@@ -40,28 +40,6 @@ def test_gaussian_filter_is_scipy_bit_for_bit(shape):
         assert np.array_equal(got.view(np.uint32), scipy_gaussian_filter(x, s).view(np.uint32)), (shape, s)
     both = R.gaussian_filter(xd, [6.0, 1.2]).cpu().numpy()
     assert np.array_equal(both[0], scipy_gaussian_filter(x, 6.0)) and np.array_equal(both[1], scipy_gaussian_filter(x, 1.2))
-
-
-def compare(got, g, parts):
-    """Assert the tolerance rule of `got` against `g` (the oracle's intermediates `parts` at the same pixels); returns
-    (boundary pixels, worst share of the bound)."""
-    assert got.shape == g.shape and got.dtype == np.float32
-    assert np.array_equal(np.isnan(got), np.isnan(g))
-    diff = np.nan_to_num(np.abs(got - g)).max(axis=-1)
-    off = diff > TOL
-    if off.any():
-        arg = parts["arg"][off].astype(np.float64) * 256
-        assert not parts["ocean"][off].any()
-        assert np.all(np.abs(arg - np.round(arg)) <= BOUNDARY), arg[np.abs(arg - np.round(arg)) > BOUNDARY][:5]
-        # the pixel is the adjacent entry across that integer, shaded with the oracle's intensity
-        k = np.round(arg).astype(np.int64)
-        idx = np.minimum(np.floor(arg).astype(np.int64), 255)
-        alt = np.clip(np.where(idx == k, k - 1, k), 0, 255)
-        lut = R.terrain_lut().astype(np.float32)
-        alt_rgb = np.clip(lut[alt] * parts["gain"][off][:, None], 0, 1)
-        assert float(np.abs(got[off] - alt_rgb).max()) <= TOL
-    share = float(diff[~off].max()) / TOL
-    return int(off.sum()), share
 
 
 @pytest.mark.parametrize("name", list(CASES))
