@@ -367,6 +367,25 @@ int tdx_flow_accumulate(const float* z, int64_t n, const int32_t* recv, const ui
  * out[h / k][w / k] (postprocessing.py:72-85); nothing to do (out may be NULL) when that is empty.  A must be 0 at
  * invalid pixels, as tdx_flow_accumulate leaves it. */
 int tdx_flow_indicator(const float* A, int32_t h, int32_t w, int32_t k, float* out, void* stream);
+/* fill_depressions_priority_flood(height, epsilon, max_raise=None, connectivity, nodata) (postprocessing.py:139-260),
+ * bit for bit, into out[h][w] (must not alias height).  A pixel is invalid when it is NaN, <= 0 or == nodata (pass NaN
+ * for no nodata; compared in fp32); seeds are the valid border pixels and the valid pixels with an invalid neighbour.
+ * Invalid pixels and seeds keep their height; every other pixel is the fixed point of
+ * out = h if h > m else max(h, m + epsilon) (fp32 add), m = min of out over its valid neighbours (connectivity 4:
+ * N, S, W, E; any other value: all 8), found by relaxing down from +inf.  epsilon is the caller's fp32 rounding of
+ * the reference's argument, finite and >= 0.  kind: DEVICE uint8[h][w] scratch; flags: DEVICE uint32[TDX_FILL_BATCH]
+ * scratch.  Runs the relaxation in batches of passes and reads a flag back after each batch, so the call synchronises
+ * `stream`; *passes (HOST, may be NULL) receives the number of relaxation passes run. */
+#define TDX_FILL_BATCH 32
+int tdx_fill_depressions(const float* height, int32_t h, int32_t w, float epsilon, int32_t connectivity, float nodata,
+                         float* out, uint8_t* kind, uint32_t* flags, int32_t* passes, void* stream);
+/* smooth_river_bumps(height, slope_thresh, smooth_strength, iterations) (postprocessing.py:87-135) into out[h][w]:
+ * `iterations` slope-weighted Laplacian steps on the NaN mask of height, each fp32 operation rounded separately in
+ * numpy's order, np.gradient central / one-sided differences, np.roll wrap-around neighbours, exp in fp64 rounded
+ * once.  slope_thresh and smooth_strength are the caller's fp32 roundings.  h, w >= 2.  scratch: DEVICE fp32[h][w],
+ * needed when iterations > 1; height, out and scratch must not alias.  iterations <= 0 copies height. */
+int tdx_smooth_river_bumps(const float* height, int32_t h, int32_t w, float slope_thresh, float smooth_strength,
+                           int32_t iterations, float* out, float* scratch, void* stream);
 
 /* Tile-seeded N(0,1) field, bit-exact with inference/portable_rng.py + world_pipeline.py:66-115 */
 int tdx_noise_patch(uint64_t base_seed, int64_t y0, int64_t x0, int32_t h, int32_t w, int32_t channels,

@@ -176,6 +176,12 @@ def _declare(l: C.CDLL) -> None:
                                       C.c_void_p]
     l.tdx_flow_indicator.restype = C.c_int
     l.tdx_flow_indicator.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+    l.tdx_fill_depressions.restype = C.c_int
+    l.tdx_fill_depressions.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_float, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p]
+    l.tdx_smooth_river_bumps.restype = C.c_int
+    l.tdx_smooth_river_bumps.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_int32,
+                                         C.c_void_p, C.c_void_p, C.c_void_p]
     l.tdx_noise_patch.restype = C.c_int
     l.tdx_noise_patch.argtypes = [C.c_uint64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                   C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]

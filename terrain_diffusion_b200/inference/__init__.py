@@ -12,6 +12,7 @@ from .stages import (coarse_epilogue, coarse_geometry, coarse_stage_tile, decode
 from .lazy_canvas import LazyCanvas, TensorWindow  # noqa: F401
 from .pipeline import TerrainPipeline, WorldPipeline  # noqa: F401
 from .relief import get_relief_map  # noqa: F401
-from .hydrology import d8_flow, flow_accumulation, plot_flow_indicator  # noqa: F401
+from .hydrology import (d8_flow, fill_depressions_priority_flood, flow_accumulation,  # noqa: F401
+                        plot_flow_indicator, smooth_river_bumps)
 from .multiphase import (build_timestep_ranges, infinite_diffusion_canvases, phase_step_ranges,  # noqa: F401
                          sample_infinite_diffusion)
