@@ -334,6 +334,28 @@ int tdx_relief_shade(const float* elev, const float* blurred, const uint32_t* st
                      int32_t vmin_is_zero, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * The explorer's detail view (explorer/server.py:188-270), which the reference renders on the host from a full get()
+ * copy.  terrain_diffusion_b200/inference/explorer.py composes the calls.  Planes are contiguous fp32 of n pixels;
+ * images are uint8 RGBA [n][4], 4-byte aligned.
+ * ------------------------------------------------------------------------------------------------------------------ */
+/* One pass over x[n] (server.py:207,214): range[0] = ~key(nanmin), range[1] = key(nanmax), where key maps a float's
+ * bits to an unsigned that orders like the float and is never 0; both 0 when every value is NaN.  range is a DEVICE
+ * uint32[2]; the call zeroes it first. */
+int tdx_detail_range(const float* x, int64_t n, uint32_t* range, void* stream);
+/* The elevation / temperature image (server.py:206-218 + _png_response :67-71): vmin, vmax from `range`
+ * (tdx_detail_range of the same x; NaN when empty), vmax = vmin + 1 in fp64 when equal; matplotlib's Normalize (every
+ * pixel 0 when vmin == vmax, else fp32((fp32(x - vmin)) / (vmax - vmin)) with each step in fp64); Colormap over lut
+ * (DEVICE fp32 [256][3]: x*256 in fp32, 256 -> 255, under -> first, over -> last, NaN -> (0, 0, 0, 0), alpha 1);
+ * clip to [0, 1]; to_rgba(bytes=True): uint8(trunc(fp32(c * 255))). */
+int tdx_detail_colour(const float* x, int64_t n, const uint32_t* range, const float* lut, uint8_t* out, void* stream);
+/* The relief image (server.py:219-228): rgb fp32 [n][3] -> concatenate([clip(rgb, 0, 1), 1]), clip, to_rgba(bytes=True);
+ * a pixel with a NaN channel is (0, 0, 0, 0). */
+int tdx_detail_rgba8(const float* rgb, int64_t n, uint8_t* out, void* stream);
+/* The /api/detail_raw body (server.py:252-260): n int16-LE elevations (tdx_post_combine's packing: floor, clip,
+ * NaN -> 0), then, when temp is not NULL, temp's n fp32-LE values bit for bit.  body: 2n (+ 4n) bytes, 2-byte aligned. */
+int tdx_detail_raw(const float* elev, const float* temp, int64_t n, void* body, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * River routing (d8_flow, flow_accumulation, plot_flow_indicator, inference/postprocessing.py:6-85), which the
  * reference runs on the CPU, the accumulation as a Python loop over every land pixel.
  * terrain_diffusion_b200/inference/hydrology.py composes the calls.  Elevations are contiguous fp32 [h][w] with h * w <= 2^24 (the largest size at

@@ -165,6 +165,14 @@ def _declare(l: C.CDLL) -> None:
     l.tdx_relief_shade.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_float, C.c_float, C.c_double, C.c_double, C.c_double, C.c_float, C.c_float,
                                    C.c_int32, C.c_float, C.c_float, C.c_int32, C.c_void_p, C.c_void_p]
+    l.tdx_detail_range.restype = C.c_int
+    l.tdx_detail_range.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    l.tdx_detail_colour.restype = C.c_int
+    l.tdx_detail_colour.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    l.tdx_detail_rgba8.restype = C.c_int
+    l.tdx_detail_rgba8.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    l.tdx_detail_raw.restype = C.c_int
+    l.tdx_detail_raw.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     l.tdx_flow_d8.restype = C.c_int
     l.tdx_flow_d8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

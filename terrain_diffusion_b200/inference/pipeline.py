@@ -473,10 +473,45 @@ class WorldPipeline:
         """Shaded relief RGB [H, W, 3] of the elevation over pixel rows [i1,i2) x columns [j1,j2): `get_elev` and then
         `get_relief_map` on the device, with `resolution` defaulting to `native_resolution` as the explorer passes it
         (server.py:219-226).  numpy for WorldPipeline, a CUDA tensor for TerrainPipeline."""
+        rgb = self._relief_on_device(i1, j1, i2, j2, **kw)
+        return rgb.cpu().numpy() if self._host_views else rgb
+
+    def _relief_on_device(self, i1: int, j1: int, i2: int, j2: int, **kw) -> torch.Tensor:
         from .relief import get_relief_map
         kw.setdefault("resolution", self.native_resolution)
-        rgb = get_relief_map(self.get_elev(i1, j1, i2, j2), None, None, None, **kw)
-        return rgb.cpu().numpy() if self._host_views else rgb
+        return get_relief_map(self.get_elev(i1, j1, i2, j2), None, None, None, **kw)
+
+    def get_detail(self, i1: int, j1: int, i2: int, j2: int, mode: str = "relief"):
+        """The explorer's `/api/detail.png` picture of pixel rows [i1, i2) x columns [j1, j2) (server.py:188-231) as the
+        uint8 RGBA [H, W, 4] that `plt.imsave` hands to the PNG encoder; the caller encodes the PNG.  mode 'elevation':
+        the elevation in the `terrain` colormap, from `get_elev` alone (the reference also computes the climate and
+        discards it); 'temperature': climate plane 0 in `RdBu_r`; any other mode: the shaded relief of `get_relief`'s
+        device path (resolution = native_resolution), NaN pixels transparent.  numpy (one pinned copy) for
+        WorldPipeline, a CUDA tensor for TerrainPipeline.
+
+        Raises ValueError before any device work for a non-integer coordinate, an empty window, more than 65535 rows,
+        or a relief window narrower than 2 pixels on either axis."""
+        from . import explorer, postproc
+        explorer.detail_window(i1, j1, i2, j2, mode)
+        if mode == "elevation":
+            img = explorer.colour_image(self.get_elev(i1, j1, i2, j2), "terrain")
+        elif mode == "temperature":
+            img = explorer.colour_image(self._get_device(i1, j1, i2, j2, True)["climate"][0], "RdBu_r")
+        else:
+            img = explorer.relief_rgba8(self._relief_on_device(i1, j1, i2, j2))
+        return postproc.to_host(img).numpy() if self._host_views else img
+
+    def detail_raw_payload(self, i1: int, j1: int, i2: int, j2: int) -> tuple:
+        """(body, (H, W), has_temp) of the explorer's `GET /api/detail_raw` (server.py:234-270): body is byte for byte
+        the handler's -- H*W int16-LE elevations (floor, clip; NaN packs as 0), then climate plane 0 as H*W fp32-LE --
+        and has_temp is its X-Has-Temp.  Packed on the device in one launch and copied to the host once.  Argument errors
+        as get_detail."""
+        from . import explorer, postproc
+        H, W = explorer.detail_window(i1, j1, i2, j2)
+        out = self._get_device(i1, j1, i2, j2, True)
+        temp = out["climate"][0] if out["climate"] is not None else None
+        body = explorer.raw_body(out["elev"], temp)
+        return postproc.to_host(body).numpy().tobytes(), (H, W), temp is not None
 
     def residual_normalized(self, i1: int, j1: int, i2: int, j2: int) -> torch.Tensor:
         """Blended decoder output over pixel rows [i1,i2) x columns [j1,j2): residual[0] / residual[1] (on the device)."""

@@ -25,18 +25,21 @@ MAX_RADIUS = 96                      # tdx_relief_gaussian's limit on int(4 sigm
 ALTITUDE_DEG = 45.0                  # sun elevation (relief_map.py:103)
 
 
+def create_lookup_table(segments) -> np.ndarray:
+    """fp64 [256]: matplotlib's `colors._create_lookup_table(256, segments, gamma=1)` for one channel's segment data,
+    rows (x, y0, y1) with x rising from 0 to 1."""
+    adata = np.array(segments, dtype=np.float64)
+    x, y0, y1 = adata[:, 0] * (LUT_SIZE - 1), adata[:, 1], adata[:, 2]
+    xind = (LUT_SIZE - 1) * np.linspace(0, 1, LUT_SIZE)
+    ind = np.searchsorted(x, xind)[1:-1]
+    distance = (xind[1:-1] - x[ind - 1]) / (x[ind] - x[ind - 1])
+    return np.clip(np.concatenate([[y1[0]], distance * (y0[ind] - y1[ind - 1]) + y1[ind - 1], [y0[-1]]]), 0.0, 1.0)
+
+
 def terrain_lut() -> np.ndarray:
     """fp64 [256, 3]: the table `LinearSegmentedColormap.from_list("terrain", _terrain_data, 256)` builds, channel by
     channel, with `colors._create_lookup_table` (gamma 1)."""
-    pos = np.array([p for p, _ in TERRAIN_STOPS], dtype=np.float64) * (LUT_SIZE - 1)
-    xind = (LUT_SIZE - 1) * np.linspace(0, 1, LUT_SIZE)
-    ind = np.searchsorted(pos, xind)[1:-1]
-    distance = (xind[1:-1] - pos[ind - 1]) / (pos[ind] - pos[ind - 1])
-    out = np.empty((LUT_SIZE, 3), dtype=np.float64)
-    for c in range(3):
-        y = np.array([rgb[c] for _, rgb in TERRAIN_STOPS], dtype=np.float64)
-        out[:, c] = np.clip(np.concatenate([[y[0]], distance * (y[ind] - y[ind - 1]) + y[ind - 1], [y[-1]]]), 0.0, 1.0)
-    return out
+    return np.stack([create_lookup_table([(p, rgb[c], rgb[c]) for p, rgb in TERRAIN_STOPS]) for c in range(3)], axis=1)
 
 
 def gaussian_taps(sigma: float) -> np.ndarray:
