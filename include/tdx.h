@@ -359,12 +359,12 @@ int tdx_detail_raw(const float* elev, const float* temp, int64_t n, void* body, 
  * River routing (d8_flow, flow_accumulation, plot_flow_indicator, inference/postprocessing.py:6-85), which the
  * reference runs on the CPU, the accumulation as a Python loop over every land pixel.
  * terrain_diffusion_b200/inference/hydrology.py composes the calls.  Elevations are contiguous fp32 [h][w] with h * w <= 2^24 (the largest size at
- * which fp32 counts are exact); a pixel is ocean (invalid) when it is NaN or <= 0.  A pixel "pushes" when it is valid,
+ * which fp32 counts are exact); a pixel is ocean (invalid) when it is NaN or <= 0, -inf included.  A pixel "pushes" when it is valid,
  * not a sink and its receiver is valid; `recv` holds the receiver's flat index for those pixels and -1 elsewhere, and
  * `indeg` the number of pixels that push into each pixel.  `flags` is a DEVICE uint32 the call zeroes and then ORs
  * TDX_FLOW_* bits into.
  * ------------------------------------------------------------------------------------------------------------------ */
-#define TDX_FLOW_INF 1            /* an elevation is +inf or -inf */
+#define TDX_FLOW_INF 1            /* an elevation is +inf (-inf is ocean and allowed) */
 #define TDX_FLOW_RANGE 2          /* a receiver index lies outside the image */
 #define TDX_FLOW_NOT_DOWNHILL 4   /* a followed edge is not strictly downhill in fp32 */
 /* d8_flow(z, tol) (postprocessing.py:6-46), bit for bit: neighbours N, S, W, E, NW, NE, SW, SE read edge-clamped,

@@ -8,8 +8,10 @@
 //   tdx_flow_accumulate  exact integer subtree sums over that forest: leaves walk downstream, and at each node only
 //                        the last child to arrive carries on, so no thread ever waits for another;
 //   tdx_flow_indicator   non-overlapping k x k max-pool and log1p.
-// A pixel is ocean (invalid) when it is NaN or <= 0.  A pixel "pushes" when it is valid, not a sink, and its receiver
-// is valid: exactly the edges flow_accumulation follows.
+// A pixel is ocean (invalid) when it is NaN or <= 0 (-inf included).  A pixel "pushes" when it is valid, not a sink,
+// and its receiver is valid: exactly the edges flow_accumulation follows.  Only +inf is flagged: a +inf pixel next to
+// another makes the reference's slope NaN (inf - inf), and its argmax then depends on where the NaN sits.  -inf is
+// ocean, so the ocean rules overwrite every slope it takes part in.
 #include "tdx_common.h"
 #include "tdx_ptx.cuh"
 
@@ -21,6 +23,7 @@ constexpr int kFlowZW = kFlowTileW + 4, kFlowZH = kFlowTileH + 4;         // ele
 constexpr unsigned char kNoPush = 0xff;
 
 __device__ __forceinline__ bool is_ocean(float v) { return isnan(v) || v <= 0.f; }
+__device__ __forceinline__ bool is_pos_inf(float v) { return v == __int_as_float(0x7f800000); }
 __device__ __forceinline__ int clampi(int v, int hi) { return v < 0 ? 0 : (v > hi ? hi : v); }
 
 struct D8Cell {
@@ -128,7 +131,7 @@ __global__ void __launch_bounds__(kFlowTileW* kFlowTileH) flow_d8_kernel(const F
   if (!inside) return;
 
   const long o = (long)y * q.w + x;
-  if (isinf(zs[ly + 2][lx + 2])) atomicOr(q.flags, (unsigned)TDX_FLOW_INF);
+  if (is_pos_inf(zs[ly + 2][lx + 2])) atomicOr(q.flags, (unsigned)TDX_FLOW_INF);
   if (q.kmax) q.kmax[o] = (int8_t)own.k;
   if (q.is_sink) q.is_sink[o] = own.sink;
   if (q.rr) q.rr[o] = own.ry;
@@ -157,7 +160,7 @@ __global__ void flow_link_kernel(const float* __restrict__ z, const int64_t* __r
   const long v = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= (long)h * w) return;
   const float c = z[v];
-  unsigned bad = isinf(c) ? (unsigned)TDX_FLOW_INF : 0u;
+  unsigned bad = is_pos_inf(c) ? (unsigned)TDX_FLOW_INF : 0u;
   const int64_t r = rr[v], s = cc[v];
   int32_t t = -1;
   if (r < 0 || r >= h || s < 0 || s >= w) {

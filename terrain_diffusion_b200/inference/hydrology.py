@@ -11,8 +11,10 @@ device computes exactly under any thread schedule: the outputs are bit-identical
 
 Conventions (as inference/relief.py): a numpy array or CPU tensor is computed on the current CUDA device and numpy is
 returned, with the reference's dtypes; a CUDA tensor returns torch tensors on its own device, computed on its current
-stream.  `z` must be a 2-D float array of at most 2^24 pixels without +-inf; it is computed in fp32 (a float64 `z` is
-rounded to fp32 first).  Argument errors raise ValueError before any device work, except the +-inf check of a CUDA
+stream.  `z` must be a 2-D float array of at most 2^24 pixels without +inf; it is computed in fp32 (a float64 `z` is
+rounded to fp32 first).  -inf is ocean, as in the reference: its slopes are all overwritten by the ocean rules.  +inf
+is rejected because a +inf pixel next to another has the NaN slope inf - inf, and the reference's argmax then depends
+on where that NaN sits.  Argument errors raise ValueError before any device work, except the +inf check of a CUDA
 tensor, which reads one 4-byte flag back after the launches.
 """
 from __future__ import annotations
@@ -37,7 +39,7 @@ def _shape(x) -> tuple:
 
 def _elevation(z, fn: str, name: str = "z", finite: bool = True):
     """(fp32 z, on_device): a contiguous CUDA tensor when z is one, else a host numpy array, after every check that
-    needs no device.  finite=False accepts +-inf."""
+    needs no device.  finite=False accepts +inf (-inf is always accepted: it is ocean)."""
     if isinstance(z, torch.Tensor):
         floating = z.is_floating_point()
     else:
@@ -55,8 +57,8 @@ def _elevation(z, fn: str, name: str = "z", finite: bool = True):
     host = z.detach().cpu().numpy() if isinstance(z, torch.Tensor) else z
     with np.errstate(over="ignore"):
         host = np.ascontiguousarray(host, dtype=np.float32)
-    if finite and np.isinf(host).any():
-        raise ValueError(f"{fn}: z has +-inf elevations (in fp32); their slopes are NaN and the result would depend on "
+    if finite and np.isposinf(host).any():
+        raise ValueError(f"{fn}: z has +inf elevations (in fp32); their slopes are NaN and the result would depend on "
                          "the visiting order")
     return host, False
 
@@ -70,7 +72,7 @@ def _on_device(host: np.ndarray) -> torch.Tensor:
 def _check_flags(flags: torch.Tensor, fn: str) -> None:
     f = int(flags)
     if f & _FLAG_INF:
-        raise ValueError(f"{fn}: z has +-inf elevations (in fp32); their slopes are NaN and the result would depend on "
+        raise ValueError(f"{fn}: z has +inf elevations (in fp32); their slopes are NaN and the result would depend on "
                          "the visiting order")
     if f & _FLAG_RANGE:
         raise ValueError(f"{fn}: a receiver index rr / cc lies outside the image")
@@ -166,7 +168,7 @@ def plot_flow_indicator(z, max_pool_kernel=1):
     """log1p of the upstream cell counts of d8_flow(z) (default tol), zero on invalid pixels, after a non-overlapping
     max_pool_kernel x max_pool_kernel max-pool that drops the remainder rows and columns (no pool for a kernel <= 1):
     fp32 [H // k, W // k], empty when k exceeds H or W, as in the reference.  Three launches on one stream; a CUDA
-    input reads back only the 4-byte +-inf flag."""
+    input reads back only the 4-byte +inf flag."""
     zz, on_device = _elevation(z, "plot_flow_indicator")
     try:
         k = operator.index(max_pool_kernel)

@@ -51,6 +51,34 @@ def _big():
     return e
 
 
+def _neg_inf():
+    # -inf ocean next to land, NaN, 0.0 and -0.0, on the border rows and columns, in all four corners, as one-pixel
+    # lakes and as a block whose inner pixels see only -inf
+    e = field(84, 40, 48, 400.0, 150.0)
+    e[5:12, 6:14] = -np.inf
+    e[8, 14] = np.nan                                         # NaN beside -inf
+    e[12, 6:10] = 0.0
+    e[12, 10:14] = -0.0
+    e[0, 20:25] = -np.inf
+    e[-1, 30:33] = -np.inf
+    e[15:19, 0] = -np.inf
+    e[22:24, -1] = -np.inf
+    e[0, 0] = e[0, -1] = e[-1, 0] = e[-1, -1] = -np.inf
+    e[25, 25] = e[30, 12] = e[33, 40] = -np.inf
+    return e
+
+
+def _neg_inf_seams():
+    # -inf on the rows and columns where the device's 32 x 8 tiles meet (rows 7 | 8, 15 | 16, columns 31 | 32, 63 | 64)
+    e = field(85, 20, 70, 300.0, 120.0)
+    e[7, 20:40] = -np.inf
+    e[16, 28:36] = -np.inf
+    e[2:18, 32] = -np.inf
+    e[8:12, 63] = -np.inf
+    e[15, 60:66] = np.nan
+    return e
+
+
 CASES = {
     # name: (elevation builder, d8 tol, max-pool kernels of the indicator)
     "mixed": (_mixed, 1e-3, (0, 1, 3)),
@@ -64,6 +92,29 @@ CASES = {
     "tol_large": (lambda: field(70, 48, 40, 500.0, 300.0), 5.0, (1,)),
     "tol_between": (_tol_between, 0.125 + 1e-9, (1,)),
     "big": (_big, 1e-3, (1, 3, 8)),
+    "neg_inf": (_neg_inf, 1e-3, (1, 3)),
+    "neg_inf_seams": (_neg_inf_seams, 1e-3, (1, 2)),
+    "neg_inf_all": (lambda: np.full((5, 6), -np.inf, np.float32), 1e-3, (1, 2)),
+}
+
+
+def _neg_inf_pits():
+    # smooth terrain with dug pits and -inf ocean: the fill keeps the ocean at -inf and routing must accept it
+    e = field(86, 56, 72, 250.0, 200.0)
+    rng = np.random.RandomState(87)
+    for _ in range(15):
+        y, x = rng.randint(3, 53), rng.randint(3, 69)
+        e[y - 2:y + 2, x - 2:x + 3] -= np.float32(rng.uniform(20, 200))
+    e[e < 5] = -np.inf
+    e[40:56, 0:12] = -np.inf
+    e.flat[rng.choice(e.size, 20, replace=False)] = np.nan
+    return e
+
+
+# routed after the reference's fill_depressions_priority_flood (default arguments): name -> (elevation builder, pools).
+# The golden stores the filled window as `<name>.filled` next to the routing outputs.
+FILLED_CASES = {
+    "neg_inf_filled": (_neg_inf_pits, (1, 2)),
 }
 
 

@@ -12,7 +12,8 @@ import torch
 from oracle import hydrology as O
 from terrain_diffusion_b200 import _lib as L
 from terrain_diffusion_b200.inference import hydrology as H
-from tests._hydrology_inputs import CASES, hydrology_case, serpentine
+from oracle import depressions as OD
+from tests._hydrology_inputs import CASES, FILLED_CASES, hydrology_case, serpentine
 
 ROOT = Path(__file__).resolve().parent.parent
 G = np.load(ROOT / "tests" / "golden" / "hydrology_golden.npz")
@@ -34,6 +35,35 @@ def test_oracle_matches_reference_golden(name):
         got, g = O.flow_indicator(z, k), G[f"{name}.ind{k}"]
         assert got.dtype == np.float32 and got.shape == g.shape
         assert ulps(got, g) <= 1, (k, ulps(got, g))        # numpy's fp32 log1p depends on the host's SIMD path
+
+
+@pytest.mark.parametrize("name", list(FILLED_CASES))
+def test_oracle_routes_the_reference_fill_of_a_neg_inf_dem(name):
+    build, pools = FILLED_CASES[name]
+    z = build()
+    filled = G[f"{name}.filled"]
+    assert np.isneginf(z).any() and np.array_equal(np.isneginf(filled), np.isneginf(z))   # the ocean stays -inf
+    assert np.array_equal(OD.fill(z)[0].view(np.uint32), filled.view(np.uint32))
+    rr, cc, is_sink, kmax = O.d8(filled)
+    assert np.array_equal(kmax, G[f"{name}.kmax"]) and np.array_equal(is_sink, G[f"{name}.is_sink"])
+    assert np.array_equal(O.accumulate(filled, rr, cc, is_sink).view(np.uint32), G[f"{name}.A"].view(np.uint32))
+    for k in pools:
+        assert ulps(O.flow_indicator(filled, k), G[f"{name}.ind{k}"]) <= 1
+
+
+def test_neg_inf_goldens_cover_the_ocean_rules():
+    # -inf centres are sinks that route north (kmax 0, the argmax of an all -inf column); land beside -inf prefers it
+    for name in ("neg_inf", "neg_inf_seams", "neg_inf_all"):
+        z, _, _ = hydrology_case(name)
+        ninf = np.isneginf(z)
+        assert ninf.any() and np.all(G[f"{name}.is_sink"][ninf]) and np.all(G[f"{name}.kmax"][ninf] == 0)
+        assert np.all(G[f"{name}.A"][ninf] == 0)
+    z, _, _ = hydrology_case("neg_inf")
+    assert np.isneginf(z[[0, 0, -1, -1], [0, -1, 0, -1]]).all()                   # all four corners
+    rr, cc, _, _ = O.d8(z)
+    beside = ~O.ocean(z) & ~G["neg_inf.is_sink"] & np.isneginf(z[rr, cc])
+    assert beside.sum() > 40                                   # land draining into -inf ocean, which is not followed
+    assert np.isnan(z[8, 14]) and np.isneginf(z[8, 13])       # NaN beside -inf
 
 
 def test_golden_cases_cover_the_branches():
@@ -63,7 +93,8 @@ def test_serpentine_is_one_long_path():
     assert a.ravel()[path[-1]] == 32 * 32 and np.all(np.diff(a.ravel()[path]) > 0)
 
 
-def test_argument_errors_come_before_any_device_work(monkeypatch):
+def test_argument_errors_and_positive_inf_come_before_any_device_work(monkeypatch):
+    # +inf (and a value that rounds to it in fp32) is refused on the host; -inf is ocean and reaches the device
     def no_device(*a, **k):
         raise AssertionError("device work before the argument checks")
 
@@ -79,14 +110,20 @@ def test_argument_errors_come_before_any_device_work(monkeypatch):
         for fn in fns[:2]:
             with pytest.raises(ValueError):
                 fn(bad)
-    for bad_value in (np.inf, -np.inf, 1e300):               # 1e300 is +inf in fp32
+    for bad_value in (np.inf, 1e300):                        # 1e300 is +inf in fp32
         zb = z.astype(np.float64)
         zb[2, 3] = bad_value
         for fn in fns:
-            with pytest.raises(ValueError):
+            with pytest.raises(ValueError, match=r"\+inf"):
                 fn(zb)
-        with pytest.raises(ValueError):
+        with pytest.raises(ValueError, match=r"\+inf"):
             H.d8_flow(torch.from_numpy(zb))                  # CPU tensor: checked on the host
+    for ocean_value in (-np.inf, -1e300):                    # -inf is ocean: it passes the host checks
+        zb = z.astype(np.float64)
+        zb[2, 3] = ocean_value
+        for fn in fns:
+            with pytest.raises(L.TdxError):
+                fn(zb)
     with pytest.raises(ValueError):
         H.flow_accumulation(z, idx[:5], idx, sink)
     with pytest.raises(ValueError):

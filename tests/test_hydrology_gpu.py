@@ -169,3 +169,20 @@ def test_infinite_elevation_on_the_device_is_an_error():
     with pytest.raises(ValueError, match="inf"):
         flow_accumulation(zd, *[torch.zeros(64, 64, dtype=torch.int64, device="cuda")] * 2,
                           torch.ones(64, 64, dtype=torch.bool, device="cuda"))
+
+
+def test_neg_inf_ocean_routes_after_the_fill():
+    from terrain_diffusion_b200.inference import fill_depressions_priority_flood
+    from tests._hydrology_inputs import FILLED_CASES
+    for name, (build, pools) in FILLED_CASES.items():
+        z = build()
+        filled = fill_depressions_priority_flood(z)
+        assert np.isneginf(filled).any()
+        assert np.array_equal(filled.view(np.uint32), G[f"{name}.filled"].view(np.uint32))
+        rr, cc, is_sink, kmax = d8_flow(filled)
+        assert np.array_equal(kmax, G[f"{name}.kmax"]) and np.array_equal(is_sink, G[f"{name}.is_sink"])
+        a = flow_accumulation(filled, rr, cc, is_sink)
+        assert np.array_equal(a.view(np.uint32), G[f"{name}.A"].view(np.uint32))
+        for k in pools:
+            ind = plot_flow_indicator(fill_depressions_priority_flood(torch.from_numpy(z).cuda()), max_pool_kernel=k)
+            assert ulps(ind.cpu().numpy(), G[f"{name}.ind{k}"]) <= 1
