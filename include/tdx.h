@@ -432,6 +432,23 @@ uint64_t tdx_tile_seed(uint64_t base_seed, int64_t ty, int64_t tx);
  * Program: a recorded sequence of the launches above with pre-built TMA descriptors, replayed as one CUDA graph.
  * This is what EDMUnet2D.forward / the N-step tile sampler become: the Python host plans the launch list once per
  * (model, batch, H, W) and then issues ONE call per forward (or per whole N-step solve).
+ *
+ * tdx_program_add_* validates the descriptor and COPIES it (for embed, also the TdxEmbedBlock array it points to):
+ * the caller may overwrite or free both as soon as add returns.  The pointers inside are recorded, not the data they
+ * point to: a graph fixes addresses, and every run reads the buffers' current contents.  A failed add changes nothing.
+ * A successful add drops the captured graph; the next graph run (or tdx_program_instantiate) captures it again.
+ * A run with use_graph != 0 on a stream that is itself capturing records the launches one by one into the caller's
+ * capture (a graph cannot be launched into a capture); tdx_program_run with use_graph == 0 and tdx_program_profile
+ * issue them one by one too.  However a program is issued, its results are bit-identical (no atomics, fixed split-K
+ * and statistics slots).
+ *
+ * Programmatic dependent launch (PDL): every launch may start while the previous one on the stream is still running.
+ * Each kernel waits for the earlier launches (griddepcontrol.wait) before it touches activations, side planes,
+ * modulation vectors, the sample / x0_prev / model_out / guide_out buffers or the split-K scratch, EXCEPT:
+ *   - igemm reads `b_packed` (the packed weights) before it waits;
+ *   - conv_out reads `weight` before it waits.
+ * These two must therefore not be written by any libtdx launch that can still be in flight on that stream (e.g. the
+ * previous launch); write them with an ordinary stream-ordered copy, or from an earlier, completed launch.
  * ------------------------------------------------------------------------------------------------------------------ */
 typedef struct TdxProgram TdxProgram;
 int tdx_program_create(TdxProgram** out);
@@ -441,7 +458,7 @@ int tdx_program_add_conv_out(TdxProgram* p, const TdxConvOutDesc* d);
 int tdx_program_add_embed(TdxProgram* p, const TdxEmbedDesc* d);
 int tdx_program_add_attn(TdxProgram* p, const TdxAttnDesc* d);
 int tdx_program_num_launches(const TdxProgram* p);
-/* use_graph != 0: capture on first run, replay afterwards. */
+/* use_graph != 0: capture on the first run after an add, replay afterwards; on a capturing stream: see above. */
 int tdx_program_run(TdxProgram* p, int use_graph, void* stream);
 /* Capture + instantiate + upload the graph without running it (keeps one-time costs out of timed regions). */
 int tdx_program_instantiate(TdxProgram* p, void* stream);

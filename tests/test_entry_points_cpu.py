@@ -12,18 +12,6 @@ CSRC = ROOT / "terrain_diffusion_b200" / "csrc"
 ALLOWLIST = {
     "tdx_debug_set_igemm_trace": "debug hook compiled only into debug builds; tools/trace_igemm.py drives it",
     "tdx_debug_set_igemm_timeline": "debug hook compiled only into debug builds; tools/timeline_forward.py drives it",
-    "tdx_igemm_packed_weight_elems": "sizes the packed weights in models/plan.py, which every model test runs",
-    "tdx_program_create": "models/plan.py builds every model forward as a program; every model test runs it",
-    "tdx_program_add_im2col": "models/plan.py records the first convolution; every model test runs it",
-    "tdx_program_add_igemm": "models/plan.py records every convolution; every model test runs it",
-    "tdx_program_add_conv_out": "models/plan.py records the last convolution; every model test runs it",
-    "tdx_program_add_embed": "models/plan.py records the embedding; every model test runs it",
-    "tdx_program_add_attn": "models/plan.py records the attention blocks; every model test runs it",
-    "tdx_program_num_launches": "models/plan.py sizes its profile buffers with it; every model test runs it",
-    "tdx_program_run": "models/plan.py replays every forward through it; every model test runs it",
-    "tdx_program_instantiate": "models/plan.py instantiates the graph before timing; every model test runs it",
-    "tdx_program_profile": "models/plan.py's per-launch profile; the planner tests run it",
-    "tdx_program_destroy": "models/plan.py frees every program; every model test runs it",
 }
 
 
