@@ -356,6 +356,37 @@ int tdx_detail_rgba8(const float* rgb, int64_t n, uint8_t* out, void* stream);
 int tdx_detail_raw(const float* elev, const float* temp, int64_t n, void* body, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * The explorer's coarse map (explorer/server.py:58-185) and the random sampler's land search
+ * (random_sampler.py:61-119), which the reference computes on the host from per-channel copies of the coarse canvas.
+ * terrain_diffusion_b200/inference/coarse_view.py composes the calls.  A canvas slice is contiguous fp32 [7][n]
+ * (sum v*w of channels 0..5, then sum w); planes are fp32 [7][n]: the six real-unit channels, then channel 4's display
+ * plane log1p(max(x, 0)).
+ * ------------------------------------------------------------------------------------------------------------------ */
+/* One pass (server.py:58-64, 113-114, 177-182; world_pipeline.py:269-274): x = v / (w + fp32(1e-8)) when eps != 0, else
+ * v / w, then sign(x) * x * x for channels 0 and 1; planes (NULL: not written) as above.  range is a DEVICE
+ * uint32[14]: per plane p, range[2p] = ~key(nanmin) and range[2p+1] = key(nanmax) as tdx_detail_range writes them
+ * (both 0 when the plane is all NaN); the call zeroes it first. */
+int tdx_coarse_readout(const float* sums, int64_t n, int32_t eps, float* planes, uint32_t* range, void* stream);
+/* The /api/coarse.png image of `channel` (server.py:112-139 + _png_response :67-71): the display plane (plane 6 for
+ * channel 4, else the channel) through Normalize with vmin, vmax from its range pair (tdx_detail_colour's rules) and
+ * lut (DEVICE fp32 [256][3]); then, where a bound fails, rgb *= fp32(0.3); clip; to_rgba(bytes=True).  bounds is a HOST
+ * fp32 [6][2] of (lo, hi) per channel, rounded to fp32 as numpy compares them; bit 2c of `active` enables
+ * `x >= lo[c]`, bit 2c+1 `x <= hi[c]` (NaN fails both); channel 1's bits must be 0.  out: uint8 [n][4], 4-byte
+ * aligned. */
+int tdx_coarse_image(const float* planes, int64_t n, int32_t channel, const uint32_t* range, const float* lut,
+                     const float* bounds, uint32_t active, uint8_t* out, void* stream);
+/* np.round(x, 2) of fp32 x[n] (server.py:159): rint(x * 100) / 100, each step in fp32. */
+int tdx_coarse_round(const float* x, int64_t n, float* out, void* stream);
+/* The land search (random_sampler.py:75-93) over elev_m fp32 [h][w] (plane 0 of tdx_coarse_readout without eps): for
+ * every window position (half + io, half + jo), io < ho = h - 2 half, jo < wo = w - 2 half, the fraction of elev_m > 0
+ * over rows [io, io + 2 half) x columns [jo, jo + 2 half), rounded to fp32 as count / (2 half)^2, compared in fp64 with
+ * `frac >= min_land_frac` (half == 0: NaN, never).  Writes rows (DEVICE int32 [h][wo], the per-row counts), mask (DEVICE
+ * uint8 [ho][wo]) and list (DEVICE int32 [1 + ho * wo]): list[0] = the number of passing positions, then their indices
+ * io * wo + jo in row-major order.  With ho <= 0 or wo <= 0 only list[0] = 0 is written (rows and mask may be NULL). */
+int tdx_coarse_land(const float* elev_m, int32_t h, int32_t w, int32_t half, double min_land_frac, int32_t* rows,
+                    uint8_t* mask, int32_t* list, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * River routing (d8_flow, flow_accumulation, plot_flow_indicator, inference/postprocessing.py:6-85), which the
  * reference runs on the CPU, the accumulation as a Python loop over every land pixel.
  * terrain_diffusion_b200/inference/hydrology.py composes the calls.  Elevations are contiguous fp32 [h][w] with h * w <= 2^24 (the largest size at

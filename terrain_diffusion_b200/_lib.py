@@ -173,6 +173,16 @@ def _declare(l: C.CDLL) -> None:
     l.tdx_detail_rgba8.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     l.tdx_detail_raw.restype = C.c_int
     l.tdx_detail_raw.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    l.tdx_coarse_readout.restype = C.c_int
+    l.tdx_coarse_readout.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    l.tdx_coarse_image.restype = C.c_int
+    l.tdx_coarse_image.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
+                                   C.c_void_p, C.c_void_p]
+    l.tdx_coarse_round.restype = C.c_int
+    l.tdx_coarse_round.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    l.tdx_coarse_land.restype = C.c_int
+    l.tdx_coarse_land.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_void_p]
     l.tdx_flow_d8.restype = C.c_int
     l.tdx_flow_d8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

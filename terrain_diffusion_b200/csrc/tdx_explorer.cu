@@ -9,22 +9,12 @@
 //   tdx_detail_raw     int16 elevation + fp32 temperature, the raw body.
 // Every fp32 / fp64 operation is explicitly rounded in the order numpy performs it (NEP 50: the float64 scalars vmin and
 // vmax promote the in-place subtraction and division to fp64, rounded once into the fp32 array).
+#include "tdx_colour.cuh"
 #include "tdx_common.h"
 #include "tdx_ptx.cuh"
 #include "tdx_upsample.cuh"
 
 namespace tdx {
-
-constexpr int kDetailLut = 256;   // rcParams['image.lut']
-
-// A float's bits mapped to an unsigned key that orders like the float (-inf < ... < -0 < +0 < ... < +inf), never 0.
-__device__ __forceinline__ unsigned ordered_key(float v) {
-  const unsigned b = __float_as_uint(v);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float key_to_float(unsigned k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
 
 // range[0] = ~key(nanmin), range[1] = key(nanmax), both atomicMax on a zeroed buffer; 0 means "no non-NaN value".
 __global__ void detail_range_kernel(const float* __restrict__ x, long n, unsigned* __restrict__ range) {
@@ -49,38 +39,18 @@ __global__ void detail_range_kernel(const float* __restrict__ x, long n, unsigne
   }
 }
 
-// ScalarMappable.to_rgba(bytes=True) of one fp32 channel in [0, 1]: uint8(trunc(fp32(x * 255))).
-__device__ __forceinline__ unsigned quantise(float c) { return (unsigned)__fmul_rn(c, 255.f); }
-__device__ __forceinline__ float clip01(float v) { return v < 0.f ? 0.f : (v > 1.f ? 1.f : v); }   // keeps NaN
-
 __global__ void detail_colour_kernel(const float* __restrict__ x, long n, const unsigned* __restrict__ range,
                                      const float* __restrict__ lut, uchar4* __restrict__ out) {
   pdl_launch_dependents();
   pdl_wait();
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  // server.py:207-209: vmin, vmax = float(nanmin), float(nanmax) (NaN for an all-NaN plane); vmax = vmin + 1 if equal
-  const float fnan = __int_as_float(0x7fc00000);
-  const double vmin = range[1] ? (double)key_to_float(~range[0]) : (double)fnan;
-  double vmax = range[1] ? (double)key_to_float(range[1]) : (double)fnan;
-  if (vmax == vmin) vmax = __dadd_rn(vmin, 1.0);
-  // Normalize.__call__: result.fill(0) when vmin == vmax (|vmin| >= 2^53 or inf), NaN pixels included; otherwise
-  // resdat -= vmin; resdat /= (vmax - vmin), each in fp64 and stored into the fp32 array
-  float t;
-  if (vmin == vmax) {
-    t = 0.f;
-  } else {
-    const float r = __double2float_rn(__dsub_rn((double)x[i], vmin));
-    t = __double2float_rn(__ddiv_rn((double)r, __dsub_rn(vmax, vmin)));
-  }
-  // Colormap.__call__: x*N in fp32, x == N -> N-1, under -> first entry, over -> last, NaN -> bad (0, 0, 0, 0); the
-  // fp64 table was rounded to fp32 by `.astype(np.float32)`.  Then _png_response's clip (a no-op on the table) and
-  // to_rgba(bytes=True); a NaN channel cannot occur.
-  float xa = __fmul_rn(t, (float)kDetailLut);
-  if (xa == (float)kDetailLut) xa = (float)(kDetailLut - 1);
+  // server.py:207-216 and Colormap.__call__ (colour_index); the fp64 table was rounded to fp32 by
+  // `.astype(np.float32)`.  Then _png_response's clip (a no-op on the table) and to_rgba(bytes=True); a NaN channel
+  // cannot occur.
+  const int idx = colour_index(x[i], range);
   uchar4 px = make_uchar4(0, 0, 0, 0);
-  if (!isnan(xa)) {
-    const int idx = xa < 0.f ? 0 : (xa >= (float)kDetailLut ? kDetailLut - 1 : (int)xa);
+  if (idx >= 0) {
     px.x = (unsigned char)quantise(clip01(lut[idx * 3 + 0]));
     px.y = (unsigned char)quantise(clip01(lut[idx * 3 + 1]));
     px.z = (unsigned char)quantise(clip01(lut[idx * 3 + 2]));

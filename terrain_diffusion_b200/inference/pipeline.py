@@ -513,6 +513,84 @@ class WorldPipeline:
         body = explorer.raw_body(out["elev"], temp)
         return postproc.to_host(body).numpy().tobytes(), (H, W), temp is not None
 
+    # ------------------------------------------------------------------ coarse map (explorer/server.py:58-185)
+    def _coarse_sums(self, ci0: int, ci1: int, cj0: int, cj1: int) -> torch.Tensor:
+        """The coarse canvas slice [7, h, w] of (sum v*w, sum w), on the device."""
+        return self._coarse[:, ci0:ci1, cj0:cj1]
+
+    def get_coarse(self, ci0: int, ci1: int, cj0: int, cj1: int, eps: bool = True):
+        """fp32 [6, h, w] real-unit planes of coarse cells [ci0, ci1) x [cj0, cj1): v / (w + 1e-8) as the explorer's
+        `_coarse_channel` divides (eps=True) or v / w as `normalize_tensor` does (eps=False), then sign(x) * x^2 for
+        channels 0 and 1 (metres).  One launch; a CPU tensor (one pinned copy) for WorldPipeline, a CUDA tensor for
+        TerrainPipeline.  Raises ValueError before any device work for a non-integer coordinate, an empty window or
+        more than 65535 rows."""
+        from . import coarse_view as CV, postproc
+        CV.coarse_window(ci0, ci1, cj0, cj1)
+        planes, _ = CV.readout(self._coarse_sums(ci0, ci1, cj0, cj1), eps)
+        return postproc.to_host(planes[:6]) if self._host_views else planes[:6]
+
+    def coarse_image(self, ci0: int, ci1: int, cj0: int, cj1: int, channel: int = 0, filters: dict | None = None,
+                     lut=None) -> tuple:
+        """(rgba8, vmin, vmax) of the explorer's `GET /api/coarse.png` (server.py:102-146): the uint8 RGBA [h, w, 4]
+        that `plt.imsave` hands to the PNG encoder, and the Python floats the handler rounds into X-Vmin / X-Vmax.
+        `channel` is shown in `lut` (default: matplotlib's viridis, read once; RuntimeError without matplotlib),
+        channel 4 as log1p(max(x, 0)), over its NaN-ignoring range.  `filters` = {channel: (lo | None, hi | None)}
+        dims to 0.3 every cell where a given bound fails (`>= lo`, `<= hi`, as numpy compares fp32 with a Python float;
+        NaN fails), as the `ch{c}_min` / `ch{c}_max` arguments do; channel 1 is ignored, as in the handler.  Two
+        launches; numpy for WorldPipeline, a CUDA tensor for TerrainPipeline.
+
+        Raises ValueError before any device work for a bad window (as get_coarse), an unknown channel, a malformed
+        filter or a lut that is not [256, 3]."""
+        from . import coarse_view as CV
+        CV.coarse_window(ci0, ci1, cj0, cj1)
+        channel = CV.check_channel(channel)
+        bounds, active = CV.filter_bounds(filters)
+        table = CV.check_lut(lut)
+        planes, rng = CV.readout(self._coarse_sums(ci0, ci1, cj0, cj1), True)
+        img = CV.image(planes, rng, channel, bounds, active, CV.lut_on(table, planes.device))
+        if self._host_views:
+            img, rng = CV.to_host_all(img, rng)
+            img = img.numpy()
+        return (img, *CV.display_range(rng, channel))
+
+    def coarse_data(self, ci0: int, ci1: int, cj0: int, cj1: int) -> dict:
+        """The dict the explorer's `GET /api/coarse_data.json` passes to `jsonify` (server.py:149-164): the window and
+        every channel's `np.round(_coarse_channel(...), 2).tolist()` by name.  Two launches and one copy.  Argument
+        errors as get_coarse."""
+        from . import coarse_view as CV, postproc
+        CV.coarse_window(ci0, ci1, cj0, cj1)
+        planes, _ = CV.readout(self._coarse_sums(ci0, ci1, cj0, cj1), True)
+        host = postproc.to_host(CV.rounded(planes)).numpy()
+        return {"ci0": ci0, "ci1": ci1, "cj0": cj0, "cj1": cj1,
+                "channels": {name: host[i].tolist() for i, name in enumerate(CV.CHANNEL_NAMES)}}
+
+    def coarse_stats(self, ci0: int, ci1: int, cj0: int, cj1: int) -> dict:
+        """The dict of the explorer's `GET /api/coarse_stats` (server.py:167-185): {channel: {'name', 'min', 'max'}}
+        with the NaN-ignoring min and max of each channel rounded to 3 decimals, from one launch and one 56-byte copy.
+        Argument errors as get_coarse."""
+        from . import coarse_view as CV, postproc
+        CV.coarse_window(ci0, ci1, cj0, cj1)
+        _, rng = CV.readout(self._coarse_sums(ci0, ci1, cj0, cj1), True, planes=False)
+        ranges = CV.range_values(postproc.to_host(rng))
+        return {ch: {"name": name, "min": round(ranges[ch][0], 3), "max": round(ranges[ch][1], 3)}
+                for ch, name in enumerate(CV.CHANNEL_NAMES)}
+
+    def land_tiles(self, coarse_window: int, detail_size: int, min_land_frac: float = 0.5) -> list:
+        """The `valid_tiles` of random_sampler.sample_land_tiles (random_sampler.py:71-93), in its order: every (ci, cj)
+        of the coarse window [-coarse_window, coarse_window)^2 whose (2 half)^2 cells around it, half =
+        (detail_size // 256) // 2, are at least `min_land_frac` land (elevation > 0 under v / w).  Four launches and one
+        copy of the list.  Raises ValueError before any device work unless coarse_window is a positive int and
+        detail_size a non-negative int; half == 0 finds nothing, as the reference's empty mean is NaN."""
+        from . import coarse_view as CV
+        if isinstance(coarse_window, bool) or not isinstance(coarse_window, (int, np.integer)) or coarse_window < 1:
+            raise ValueError(f"coarse_window must be a positive int, got {coarse_window!r}")
+        cw = int(coarse_window)
+        CV.coarse_window(-cw, cw, -cw, cw)
+        half = CV.land_half(detail_size)
+        min_land_frac = float(min_land_frac)
+        planes, _ = CV.readout(self._coarse_sums(-cw, cw, -cw, cw), False)
+        return CV.land_positions(planes[0], half, min_land_frac, -cw, -cw)
+
     def residual_normalized(self, i1: int, j1: int, i2: int, j2: int) -> torch.Tensor:
         """Blended decoder output over pixel rows [i1,i2) x columns [j1,j2): residual[0] / residual[1] (on the device)."""
         r = self._residual[:, i1:i2, j1:j2]
