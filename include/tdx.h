@@ -498,6 +498,43 @@ int tdx_program_instantiate(TdxProgram* p, void* stream);
 int tdx_program_profile(TdxProgram* p, float* ms_per_launch, int32_t* kinds, void* stream);
 int tdx_program_destroy(TdxProgram* p);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * FastNoiseLite Perlin + FBm noise and the coarse stage's synthetic conditioning map (inference/synthetic_map.py:182-271,
+ * perlin_transform.py:42-45), which the reference evaluates on the host with pyfastnoiselite.
+ * terrain_diffusion_b200/inference/synthetic_map.py and inference/minecraft.py compose the calls.  Cell (r, c) of an
+ * [h][w] window sits at x = np.arange(j0, j0 + w, dtype=np.float32)[c], y = np.arange(i0, i0 + h, dtype=np.float32)[r].
+ * Noise follows FastNoiseLite's 2-D Perlin with FBm fractal (weighted strength 0) in fp32 with every operation rounded
+ * on its own (no FMA).  Results are only defined while |x * frequency * lacunarity^(octaves - 1)| (and y) stay below
+ * 2^31.  h, w in 1..2^24 and h * w <= 2^31.
+ * ------------------------------------------------------------------------------------------------------------------ */
+#define TDX_FBM_MAX_PLANES 8
+#define TDX_SYNTH_MAX_KNOTS 512
+#define TDX_SYNTH_FINALIZE 1      /* synthetic_map.py:232-254 `finalize` on the five channels */
+#define TDX_SYNTH_SQRT0 2         /* np.sign(x) * np.sqrt(np.abs(x)) on channel 0 (+0 for either zero, NaN stays) */
+#define TDX_SYNTH_IMPORT 4        /* merge the imported rasters into the raw map (world_pipeline.py:829-880) */
+#define TDX_SYNTH_RAW_INPUT 8     /* `input` holds the raw map itself: no noise, no quantile transform */
+/* n_planes (1..TDX_FBM_MAX_PLANES) planes, plane k of the generator (seeds[k], frequency[k], octaves[k] in 1..16,
+ * lacunarity[k], gain[k]) -- HOST arrays, the float ones as FastNoiseLite stores them -- into out (DEVICE fp32
+ * [n_planes][h][w]). */
+int tdx_fbm_perlin(int32_t n_planes, const int32_t* seeds, const float* frequency, const int32_t* octaves,
+                   const float* lacunarity, const float* gain, int64_t i0, int64_t j0, int32_t h, int32_t w, float* out,
+                   void* stream);
+/* The [5][h][w] conditioning window into out (DEVICE fp32).  Per cell: the five generators of synthetic_map.py:219-225
+ * (seeds, frequency: HOST int32 / fp32 [5]; octaves 4, 2, 4, 4, 4, lacunarity 2, gain 0.5) -- or, when input (DEVICE
+ * fp32 [5][h][w]) is given, its values instead -- each through np.interp on its table pair (tables: DEVICE fp64
+ * [5][2][n_knots], noise quantiles then data quantiles, strictly increasing; left / right = the end values), in fp64,
+ * then cast to fp32.  With TDX_SYNTH_RAW_INPUT, input is taken as that fp32 raw map and tables, seeds and frequency are
+ * not read.  Then, as `mode` sets them: TDX_SYNTH_IMPORT replaces channel f of absolute cell (i0 + r, j0 + c) by
+ * imp_values[f][(i0 + r - oi) * cols + (j0 + c - oj)] inside the raster (imp_values: HOST array of 5 DEVICE fp32
+ * pointers, NULL for none; imp_boxes: HOST int64 [5][4] = oi, oj, rows, cols) and elsewhere by imp_defaults[f] (HOST fp32
+ * [5]) when bit f of imp_has_default is set; TDX_SYNTH_FINALIZE with scalars (HOST fp32 [5]: a_temp_std, b_temp_std,
+ * temp_std_p1, temp_std_p99 each rounded to fp32, and fp32(p99 - p1) with the difference taken in fp64); then
+ * TDX_SYNTH_SQRT0. */
+int tdx_synthetic_map(const double* tables, int32_t n_knots, const int32_t* seeds, const float* frequency,
+                      const float* scalars, int64_t i0, int64_t j0, int32_t h, int32_t w, const float* input,
+                      int32_t mode, const float* const* imp_values, const int64_t* imp_boxes, const float* imp_defaults,
+                      uint32_t imp_has_default, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -183,6 +183,13 @@ def _declare(l: C.CDLL) -> None:
     l.tdx_coarse_land.restype = C.c_int
     l.tdx_coarse_land.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p]
+    l.tdx_fbm_perlin.restype = C.c_int
+    l.tdx_fbm_perlin.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                 C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+    l.tdx_synthetic_map.restype = C.c_int
+    l.tdx_synthetic_map.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
+                                    C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_uint32, C.c_void_p, C.c_void_p]
     l.tdx_flow_d8.restype = C.c_int
     l.tdx_flow_d8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

@@ -6,12 +6,14 @@ climate variables and classifies every pixel into a Minecraft biome id with ~150
 host.  Here one launch of csrc/tdx_biome.cu (`tdx_minecraft_readout`) does all of it per output pixel and writes the
 fp32 planes, the int16 biome ids and/or the wire body.
 
-Noise is injected, like the conditioning map: `noise_fn(cfg, i0, j0, h, w) -> fp32 [h, w]` (numpy array or tensor)
+Noise is injected: `noise_fn(cfg, i0, j0, h, w) -> fp32 [h, w]` (numpy array or tensor)
 returns the generator of configuration `cfg` (a `NoiseConfig`) at x = j0 + c, y = i0 + r for row r, column c, as the
 reference calls `gen_from_coords`.  The reference's seven FastNoiseLite generators have five distinct configurations
 (`_TEMP_NOISE` = `_SNOW_NOISE`, `_TEMP_NOISE_FINE` = `_SNOW_NOISE_FINE`), so a request calls the provider once per
 configuration it needs: a provider must be a pure function of its arguments.  The default provider builds the
-reference's generators with pyfastnoiselite.
+reference's generators with pyfastnoiselite.  `device_noise` computes them on the device instead (csrc/tdx_synth.cu,
+FastNoiseLite's Perlin FBm restated bit for bit; see inference/synthetic_map.py), and a request given it fills every
+noise plane it needs with one launch straight into the read-out's noise buffer.
 """
 from __future__ import annotations
 
@@ -62,6 +64,14 @@ def fastnoiselite_noise(cfg: NoiseConfig, i0: int, j0: int, h: int, w: int) -> n
     return g.gen_from_coords(np.array([xx.ravel(), yy.ravel()], dtype=np.float32)).astype(np.float32).reshape(h, w)
 
 
+def device_noise(cfg: NoiseConfig, i0: int, j0: int, h: int, w: int) -> torch.Tensor:
+    """A `noise_fn` on the current CUDA device: the FastNoiseLite Perlin FBm generator of `cfg` at x = j0 + c,
+    y = i0 + r as a CUDA fp32 [h, w] tensor (inference/synthetic_map.fbm_perlin).  `request` recognises it and writes
+    all the planes of a request with one launch."""
+    from .synthetic_map import fbm_perlin
+    return fbm_perlin(cfg.seed, cfg.frequency, cfg.octaves, cfg.lacunarity, cfg.gain, i0, j0, h, w)
+
+
 def minecraft_window(i1: int, j1: int, i2: int, j2: int, scale: int):
     """Checks a request's arguments as `terrain_window` does (integers only, scale >= 1, non-empty, at most 65535 rows;
     ValueError) and returns the window the elevation is read from and the crop origin in its (upsampled) version:
@@ -84,8 +94,14 @@ def _noise_scale(noise) -> float:
 
 def noise_planes(noise_fn, i1: int, j1: int, H: int, W: int, which, device) -> torch.Tensor:
     """fp32 [5, H, W] on `device`: planes `which` (indices into NOISE_CONFIGS) from one call of `noise_fn` each, the
-    others zero."""
+    others zero.  For `device_noise`, one tdx_fbm_perlin launch writes the planes `which` (a contiguous range)."""
     out = torch.zeros((5, H, W), dtype=torch.float32, device=device)
+    if noise_fn is device_noise and which:
+        from .synthetic_map import fbm_planes
+        lo, hi = min(which), max(which) + 1
+        assert tuple(which) == tuple(range(lo, hi)), which
+        fbm_planes([NOISE_CONFIGS[k] for k in which], i1, j1, H, W, out[lo:hi])
+        return out
     for k in which:
         v = torch.as_tensor(noise_fn(NOISE_CONFIGS[k], i1, j1, H, W))
         if tuple(v.shape) != (H, W):

@@ -9,10 +9,14 @@ cache_limit=..., **kw)`, `.to(device)`, `.bind(hdf5_file)`, `.get(i1, j1, i2, j2
 `.coarse / .latents / .residual` (un-normalised (sum x w, sum w) fp32 CPU tensors, negative indices legal) and the small
 state API; all of that is here with the reference's argument names and return conventions.
 
-Outside the hot-path scope (SURVEY.md section 2) and therefore injected, not rebuilt: the synthetic conditioning map of
-the coarse stage (`synthetic_map.py`, Perlin noise + WorldClim rasters).  Pass `conditioning_fn(i1, i2, j1, j2) ->
-[5, i2-i1, j2-j1]` (what `_conditioning_model_input` returns) or provide every channel through
-`set_custom_conditioning_import`; without either the first coarse tile raises.  `caching_strategy='indirect'` (HDF5 tile
+The synthetic conditioning map of the coarse stage (`synthetic_map.py`: five Perlin FBm fields quantile-matched to
+Earth statistics) is built on the device per window when `synthetic_map_stats=` is given: the reference's statistics
+cache (`data/global/synthetic_map_stats.json`) or its mapping (see inference/synthetic_map.py; computing the statistics
+from the WorldClim rasters is not part of this package).  Imports then follow the reference's semantics (raw units,
+merged into the Perlin raw map, no finalize, sign(x) sqrt|x| of channel 0 only).  Alternatively inject
+`conditioning_fn(i1, i2, j1, j2) -> [5, i2-i1, j2-j1]` (what `_conditioning_model_input` returns) or provide every
+channel through `set_custom_conditioning_import`; with none of them the first coarse tile raises.  Passing both
+`conditioning_fn` and `synthetic_map_stats` is a ValueError.  `caching_strategy='indirect'` (HDF5 tile
 store) is not implemented -- the window cache is the byte-limited HBM LRU of `LazyCanvas` (`cache_limit`, like the
 reference's MemoryTileStore).  `torch_compile` is accepted and ignored: every U-Net evaluation already is one CUDA
 graph of hand-written kernels.
@@ -78,10 +82,12 @@ class WorldPipeline:
                  coarse_means: list | None = None, coarse_stds: list | None = None, caching_strategy: str = "direct",
                  cache_limit: int | None = 100 * 1024 * 1024, onestep_latent: bool = False,
                  decoder_tile_size: int = 512, decoder_tile_stride: int = 384, conditioning_fn=None,
-                 **deprecated_kwargs):
+                 synthetic_map_stats=None, **deprecated_kwargs):
         from .noise import next_seed
         if T not in (1, 2):
             raise ValueError(f"T must be 1 or 2, got {T}")
+        if conditioning_fn is not None and synthetic_map_stats is not None:
+            raise ValueError("pass either conditioning_fn or synthetic_map_stats, not both")
         coarse_geometry(coarse_pooling)                  # ValueError unless it divides 64 and 48 (world_pipeline.py:969-970)
         coarse_pooling = operator.index(coarse_pooling)
         self.T = T
@@ -121,6 +127,13 @@ class WorldPipeline:
         self.custom_conditioning_default_values: dict = {}
         self._host_views = True
         self._set_cond(self.kwargs["cond_snr"])
+        # the device synthesis of the conditioning map (never written to config.json: synthetic_map_stats may be a
+        # host path); its five noise seeds derive from the world seed as the reference's `_init_conditioning` does
+        self._synthetic = None
+        self._synthetic_imports = None
+        if synthetic_map_stats is not None:
+            from .synthetic_map import SyntheticMap
+            self._synthetic = SyntheticMap(synthetic_map_stats, self.kwargs["frequency_mult"], seed=self.seed)
 
     # ------------------------------------------------------------------ construction (world_pipeline.py:470-565)
     @classmethod
@@ -227,10 +240,11 @@ class WorldPipeline:
     def set_custom_conditioning_import(self, channel: int, values, origin_i: int, origin_j: int,
                                        default_value: float | None = None) -> None:
         """Install a 2-D raster for conditioning channel 0..4, `values[0, 0]` anchored at conditioning cell
-        (origin_i, origin_j); outside its footprint the channel keeps `conditioning_fn`'s value unless `default_value`
-        is given (world_pipeline.py:781-819).  The raster is overlaid as is, in MODEL-INPUT units: the unit transforms
-        the reference applies while merging imports with its Perlin maps belong to the conditioning synthesis, which is
-        the caller's here.  Calls rebuild()."""
+        (origin_i, origin_j); outside its footprint the channel keeps the synthesised value unless `default_value` is
+        given (world_pipeline.py:781-819).  With `synthetic_map_stats` the reference's semantics hold: the raster is in
+        raw units, merged into the Perlin raw map, and then only channel 0 goes through sign(x) sqrt|x| (no finalize);
+        the raster is copied to the device once.  With `conditioning_fn` it is overlaid on that function's output as
+        is, in MODEL-INPUT units.  Calls rebuild()."""
         values = np.asarray(values, dtype=np.float32)
         if values.ndim != 2:
             raise ValueError("Custom conditioning import must be a 2-D array.")
@@ -243,15 +257,22 @@ class WorldPipeline:
             self.custom_conditioning_default_values.pop(channel, None)
         else:
             self.custom_conditioning_default_values[channel] = float(default_value)
+        self._synthetic_imports = None
         self.rebuild()
 
     def rebuild(self) -> None:
-        """Drop every cached window (world_pipeline.py:714-741; call after changing seed / kwargs that affect tiles)."""
+        """Drop every cached window (world_pipeline.py:714-741; call after changing seed / kwargs that affect tiles).
+        With `synthetic_map_stats`, the five noise seeds are derived again from the world seed (a seed of 0 draws new
+        ones from `random`, as the reference's `_init_conditioning` does)."""
+        if self._synthetic is not None:
+            self._synthetic.reseed(self.seed)
         self.empty_cache()
 
     def _conditioning_model_input(self, i1: int, i2: int, j1: int, j2: int) -> torch.Tensor:
         """[5, i2-i1, j2-j1] raw conditioning map of coarse cells [i1,i2) x [j1,j2) (what the reference's
         `_conditioning_model_input` returns): the injected function, with imported rasters overlaid."""
+        if self._synthetic is not None:
+            return self._synthetic.conditioning(i1, i2, j1, j2, self._device_imports(), device=self.device)
         covered = all(ch in self.custom_conditioning_default_values for ch in range(5)) and \
             len(self.custom_conditioning_imports) == 5
         if self.conditioning_fn is not None:
@@ -271,6 +292,19 @@ class WorldPipeline:
             if a < b and c < d:
                 base[ch, a - i1:b - i1, c - j1:d - j1] = arr[a - oi:b - oi, c - oj:d - oj]
         return base
+
+    def _device_imports(self):
+        """The imported rasters on the device, in tdx_synthetic_map's form (None without imports); copied once after
+        each set_custom_conditioning_import."""
+        if not self.custom_conditioning_imports:
+            return None
+        dev = self.device
+        if self._synthetic_imports is None or self._synthetic_imports[0] != dev:
+            from .synthetic_map import device_imports
+            self._synthetic_imports = (dev, device_imports(self.custom_conditioning_imports,
+                                                           self.custom_conditioning_import_origins,
+                                                           self.custom_conditioning_default_values, dev))
+        return self._synthetic_imports[1]
 
     # ------------------------------------------------------------------ hierarchy (world_pipeline.py:961-1270)
     def _canvas(self, name, *a, **k):
@@ -354,13 +388,15 @@ class WorldPipeline:
 
     def change_seed(self, seed: int | None = None) -> bool:
         """New world seed (masked to 64 bits; None draws one like portable_rng.next_seed(None)) and all cached tiles
-        dropped; False (no-op) when the seed is unchanged.  A seed-dependent `conditioning_fn` must read
-        `pipeline.seed` itself -- the conditioning synthesis is the caller's."""
+        dropped; False (no-op) when the seed is unchanged.  With `synthetic_map_stats` the five noise seeds follow the
+        new seed; a seed-dependent `conditioning_fn` must read `pipeline.seed` itself."""
         from .noise import next_seed
         new_seed = (int(seed) & 0xFFFFFFFFFFFFFFFF) if seed is not None else next_seed(None)
         if new_seed == self.seed:
             return False
         self.seed = new_seed
+        if self._synthetic is not None:
+            self._synthetic.reseed(self.seed)
         self.empty_cache()
         return True
 
@@ -598,15 +634,18 @@ class WorldPipeline:
 
 
 class TerrainPipeline(WorldPipeline):
-    """Device-resident variant for callers that stay on the GPU: live models + an injected conditioning function in
-    the constructor, bound immediately, `.coarse / .latents / .residual / .get` return CUDA tensors."""
+    """Device-resident variant for callers that stay on the GPU: live models + a conditioning source (an injected
+    `conditioning_fn` or `synthetic_map_stats` for the device synthesis) in the constructor, bound immediately,
+    `.coarse / .latents / .residual / .get` return CUDA tensors."""
 
-    def __init__(self, coarse_model, base_model, decoder_model, seed: int, conditioning_fn, *, coarse_means, coarse_stds,
+    def __init__(self, coarse_model, base_model, decoder_model, seed: int, conditioning_fn=None, *, coarse_means,
+                 coarse_stds,
                  cond_snr, histogram_raw, latents_means, latents_stds, latents_batch_size: int = 16,
                  decoder_tile_size: int = 512, decoder_tile_stride: int = 384, latent_compression: int = 8,
                  t_inter: float | None = None, residual_mean: float | None = None, residual_std: float | None = None,
                  native_resolution: float = 90.0, cache_limit: int | None = None, coarse_pooling: int = 1,
-                 elev_coarse_pool_mode: str = "avg", p5_coarse_pool_mode: str = "avg"):
+                 elev_coarse_pool_mode: str = "avg", p5_coarse_pool_mode: str = "avg", synthetic_map_stats=None,
+                 frequency_mult: list | None = None):
         super().__init__(seed=seed, latents_batch_size=latents_batch_size, native_resolution=native_resolution,
                          latent_compression=latent_compression, cond_snr=[float(v) for v in cond_snr],
                          coarse_pooling=coarse_pooling, elev_coarse_pool_mode=elev_coarse_pool_mode,
@@ -614,6 +653,7 @@ class TerrainPipeline(WorldPipeline):
                          coarse_means=[float(v) for v in coarse_means], coarse_stds=[float(v) for v in coarse_stds],
                          cache_limit=cache_limit, decoder_tile_size=decoder_tile_size,
                          decoder_tile_stride=decoder_tile_stride, conditioning_fn=conditioning_fn,
+                         synthetic_map_stats=synthetic_map_stats, frequency_mult=frequency_mult,
                          histogram_raw=[float(v) for v in torch.as_tensor(histogram_raw).flatten()],
                          cond_input_mean=[float(v) for v in torch.as_tensor(latents_means).flatten()],
                          cond_input_std=[float(v) for v in torch.as_tensor(latents_stds).flatten()], t_inter=t_inter)

@@ -16,8 +16,9 @@ around the U-Net, `.item()`, D2H -- is organised here around ONE fused program p
                        packed output are one launch (tdx_coarse_epilogue).
 
 Noise comes from the bit-compatible GPU generator (same seeds as the reference), nothing synchronises with the host and
-nothing leaves the GPU.  Taken as arguments, because the reference computes them outside the hot path: the synthetic
-conditioning map of the coarse stage and the blended dependency windows the canvas engine hands to each callback.
+nothing leaves the GPU.  Taken as arguments: the synthetic conditioning map of the coarse stage (built on the device by
+inference/synthetic_map.py, or by a caller's `conditioning_fn`) and the blended dependency windows the canvas engine
+hands to each callback.
 """
 from __future__ import annotations
 
@@ -240,8 +241,8 @@ def coarse_stage_tile(model, scheduler, seed: int, ctx, synthetic_map: torch.Ten
                       pool_size: int = 1, elev_pool_mode: str = "avg", p5_pool_mode: str = "avg") -> torch.Tensor:
     """Coarse window (0, i, j): 20-step DPM-Solver++ solve conditioned on the noised synthetic map
     (world_pipeline.py:909-959).  synthetic_map: the raw [5, 64, 64] conditioning of conditioning cells
-    (48 i .. 48 i + 64, 48 j .. 48 j + 64) whatever the pooling (built by the reference's Perlin / WorldClim machinery,
-    out of scope).  Returns the packed [7, 64/p, 64/p] tile, p = pool_size (see coarse_geometry / coarse_epilogue);
+    (48 i .. 48 i + 64, 48 j .. 48 j + 64) whatever the pooling, a CUDA or CPU tensor (the pipeline's device synthesis,
+    inference/synthetic_map.py, or its `conditioning_fn`).  Returns the packed [7, 64/p, 64/p] tile, p = pool_size (see coarse_geometry / coarse_epilogue);
     weight_window is the [64/p, 64/p] blend window."""
     coarse_geometry(pool_size)                                   # argument errors before any device work
     dev = model.device
