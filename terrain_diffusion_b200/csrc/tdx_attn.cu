@@ -119,10 +119,7 @@ int attn_launch(const TdxAttnDesc& d, cudaStream_t stream) {
   p.tokens = d.tokens;
   p.C8 = d.heads * 8;
   const int threads = d.tokens < 256 ? ((d.tokens + 31) / 32) * 32 : 256;
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3(d.heads, d.n_img), dim3(threads), (size_t)d.tokens * 65 * 3 * 4, stream);
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attn_kernel, p));
+  TDX_CHECK_CUDA(launch(attn_kernel, dim3(d.heads, d.n_img), threads, (size_t)d.tokens * 65 * 3 * 4, stream, p));
   return TDX_OK;
 }
 

@@ -277,9 +277,6 @@ extern "C" int tdx_minecraft_readout(const float* elev, int32_t h, int32_t w, in
   p.detail = detail != 0;
   p.r = (float)(1.0 / scale);
   p.amp_c = amp_c; p.amp_f = amp_f; p.psm = pixel_size_m; p.native_res = native_res; p.slope_div = slope_div;
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3((W + 127) / 128, H), dim3(128), 0, reinterpret_cast<cudaStream_t>(stream));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, minecraft_readout_kernel, p));
+  TDX_CHECK_CUDA(launch(minecraft_readout_kernel, dim3((W + 127) / 128, H), 128, 0, stream, p));
   return TDX_OK;
 }

@@ -200,15 +200,6 @@ __global__ void __launch_bounds__(kCompactThreads) land_compact_kernel(const uin
   if (threadIdx.x == 0) list[0] = base;
 }
 
-template <typename Kernel, typename... Args>
-int launch_cells(Kernel kernel, long n, cudaStream_t stream, Args... args) {   // one thread per cell, 256 per block
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, stream);
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, args...));
-  return TDX_OK;
-}
-
 }  // namespace
 }  // namespace tdx
 
@@ -222,11 +213,8 @@ extern "C" int tdx_coarse_readout(const float* sums, int64_t n, int32_t eps, flo
   TDX_CHECK_CUDA(cudaMemsetAsync(range, 0, 2 * kPlanes * sizeof(uint32_t), st));
   const long blocks = (n + 255) / 256;
   const int grid = (int)(blocks < 4L * sm_count() ? blocks : 4L * sm_count());
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3(grid), dim3(256), 0, st);
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, coarse_readout_kernel, sums, (long)n, (int)(eps != 0), planes,
-                                    reinterpret_cast<unsigned*>(range)));
+  TDX_CHECK_CUDA(launch(coarse_readout_kernel, grid, 256, 0, st, sums, (long)n, (int)(eps != 0), planes,
+                        reinterpret_cast<unsigned*>(range)));
   return TDX_OK;
 }
 
@@ -245,14 +233,16 @@ extern "C" int tdx_coarse_image(const float* planes, int64_t n, int32_t channel,
     f.hi[c] = bounds[2 * c + 1];
   }
   f.active = active;
-  return launch_cells(coarse_image_kernel, (long)n, reinterpret_cast<cudaStream_t>(stream), planes, (long)n,
-                      (int)channel, reinterpret_cast<const unsigned*>(range), lut, f, reinterpret_cast<uchar4*>(out));
+  TDX_CHECK_CUDA(launch(coarse_image_kernel, (unsigned)((n + 255) / 256), 256, 0, stream, planes, (long)n, (int)channel,
+                        reinterpret_cast<const unsigned*>(range), lut, f, reinterpret_cast<uchar4*>(out)));
+  return TDX_OK;
 }
 
 extern "C" int tdx_coarse_round(const float* x, int64_t n, float* out, void* stream) {
   TDX_REQUIRE(x && out, "coarse_round: null pointer");
   TDX_REQUIRE(n >= 1, "coarse_round: empty input");
-  return launch_cells(coarse_round_kernel, (long)n, reinterpret_cast<cudaStream_t>(stream), x, (long)n, out);
+  TDX_CHECK_CUDA(launch(coarse_round_kernel, (unsigned)((n + 255) / 256), 256, 0, stream, x, (long)n, out));
+  return TDX_OK;
 }
 
 extern "C" int tdx_coarse_land(const float* elev_m, int32_t h, int32_t w, int32_t half, double min_land_frac,
@@ -268,16 +258,11 @@ extern "C" int tdx_coarse_land(const float* elev_m, int32_t h, int32_t w, int32_
   }
   TDX_REQUIRE(rows && mask, "coarse_land: null pointer");
   TDX_REQUIRE((long)h * wo < (1L << 31), "coarse_land: %d x %ld positions overflow the int32 list", (int)h, wo);
-  int rc = launch_cells(land_rows_kernel, (long)h * wo, st, elev_m, (int)h, (int)w, (int)half, (int)wo,
-                        reinterpret_cast<int*>(rows));
-  if (rc != TDX_OK) return rc;
-  rc = launch_cells(land_mask_kernel, ho * wo, st, reinterpret_cast<const int*>(rows), (int)ho, (int)wo, (int)half,
-                    min_land_frac, mask);
-  if (rc != TDX_OK) return rc;
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3(1), dim3(kCompactThreads), 0, st);
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, land_compact_kernel, (const uint8_t*)mask, ho * wo,
-                                    reinterpret_cast<int*>(list)));
+  TDX_CHECK_CUDA(launch(land_rows_kernel, (unsigned)(((long)h * wo + 255) / 256), 256, 0, st, elev_m, (int)h, (int)w,
+                        (int)half, (int)wo, reinterpret_cast<int*>(rows)));
+  TDX_CHECK_CUDA(launch(land_mask_kernel, (unsigned)((ho * wo + 255) / 256), 256, 0, st,
+                        reinterpret_cast<const int*>(rows), (int)ho, (int)wo, (int)half, min_land_frac, mask));
+  TDX_CHECK_CUDA(launch(land_compact_kernel, 1, kCompactThreads, 0, st, (const uint8_t*)mask, ho * wo,
+                        reinterpret_cast<int*>(list)));
   return TDX_OK;
 }

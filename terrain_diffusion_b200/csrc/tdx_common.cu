@@ -2,7 +2,6 @@
 #include "tdx_common.h"
 
 #include <cudaTypedefs.h>
-#include <string.h>
 
 namespace tdx {
 
@@ -37,19 +36,6 @@ bool first_use_on_device(bool (&seen)[16]) {
   if (seen[dev]) return false;
   seen[dev] = true;
   return true;
-}
-
-void fill_launch_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, dim3 grid, dim3 block, size_t smem,
-                        cudaStream_t stream) {
-  memset(cfg, 0, sizeof(*cfg));
-  cfg->gridDim = grid;
-  cfg->blockDim = block;
-  cfg->dynamicSmemBytes = smem;
-  cfg->stream = stream;
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg->attrs = attr;
-  cfg->numAttrs = 1;
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,

@@ -177,11 +177,8 @@ extern "C" int tdx_fill_depressions(const float* height, int32_t h, int32_t w, f
   TDX_REQUIRE(out != height, "fill_depressions: out must not alias height");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long n = (long)h * w;
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st);
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, fill_classify_kernel, height, (int)h, (int)w, (int)(connectivity != 4),
-                                    nodata, kind, out));
+  TDX_CHECK_CUDA(launch(fill_classify_kernel, (unsigned)((n + 255) / 256), 256, 0, st, height, (int)h, (int)w,
+                        (int)(connectivity != 4), nodata, kind, out));
   FillParams q;
   q.h = height; q.kind = kind; q.out = out; q.flags = flags; q.H = h; q.W = w; q.eps = epsilon;
   q.tiles_x = (w + kFillTile - 1) / kFillTile;
@@ -194,8 +191,8 @@ extern "C" int tdx_fill_depressions(const float* height, int32_t h, int32_t w, f
   long total = 0;
   for (int batch = 4;; batch = batch * 2 > TDX_FILL_BATCH ? TDX_FILL_BATCH : batch * 2) {
     TDX_CHECK_CUDA(cudaMemsetAsync(flags, 0, batch * sizeof(uint32_t), st));
-    fill_launch_config(&cfg, attr, dim3((unsigned)tiles), dim3(kFillTile * kFillRows), 0, st);
-    for (int p = 0; p < batch; ++p) TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, relax, q, p));
+    for (int p = 0; p < batch; ++p)
+      TDX_CHECK_CUDA(launch(relax, (unsigned)tiles, kFillTile * kFillRows, 0, st, q, p));
     TDX_CHECK_CUDA(cudaMemcpyAsync(seen, flags, batch * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     TDX_CHECK_CUDA(cudaStreamSynchronize(st));
     int p = 0;
@@ -225,14 +222,11 @@ extern "C" int tdx_smooth_river_bumps(const float* height, int32_t h, int32_t w,
     return TDX_OK;
   }
   TDX_REQUIRE(iterations == 1 || scratch, "smooth_river_bumps: %d iterations need a scratch plane", iterations);
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st);
   const float* src = height;
   for (int k = 0; k < iterations; ++k) {
     float* dst = (iterations - 1 - k) % 2 == 0 ? out : scratch;   // the last iteration lands in out
-    TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, smooth_step_kernel, height, src, dst, (int)h, (int)w, slope_thresh,
-                                      smooth_strength));
+    TDX_CHECK_CUDA(launch(smooth_step_kernel, (unsigned)((n + 255) / 256), 256, 0, st, height, src, dst, (int)h,
+                          (int)w, slope_thresh, smooth_strength));
     src = dst;
   }
   return TDX_OK;

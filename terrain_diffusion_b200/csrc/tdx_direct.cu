@@ -108,14 +108,11 @@ int im2col_launch(const TdxIm2colDesc& d, cudaStream_t stream) {
   p.kpad8 = d.k_pad / 8;
   p.H = d.height;
   p.W = d.width;
-  dim3 grid((d.height * d.width + 127) / 128, d.n_img);
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, grid, dim3(128), 0, stream);
-  if (p.ci == 2) TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, im2col_in_kernel<2>, p));
-  else if (p.ci == 5) TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, im2col_in_kernel<5>, p));
-  else if (p.ci == 6) TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, im2col_in_kernel<6>, p));
-  else TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, im2col_in_kernel<12>, p));
+  auto kernel = p.ci == 2 ? im2col_in_kernel<2>
+                : p.ci == 5 ? im2col_in_kernel<5>
+                : p.ci == 6 ? im2col_in_kernel<6>
+                            : im2col_in_kernel<12>;
+  TDX_CHECK_CUDA(launch(kernel, dim3((d.height * d.width + 127) / 128, d.n_img), 128, 0, stream, p));
   return TDX_OK;
 }
 
@@ -294,16 +291,9 @@ int conv_out_launch(const TdxConvOutDesc& d, cudaStream_t stream) {
   int rc_prep = direct_prepare();
   if (rc_prep != TDX_OK) return rc_prep;
   dim3 grid((d.height * d.width + 32 * kConvOutGroups - 1) / (32 * kConvOutGroups), d.n_img);
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, grid, dim3(128), smem, stream);
-  if (d.guide_out) {
-    if (wout == 1) TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_out_kernel<1, true>, p));
-    else TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_out_kernel<8, true>, p));
-  } else {
-    if (wout == 1) TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_out_kernel<1, false>, p));
-    else TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_out_kernel<8, false>, p));
-  }
+  auto kernel = d.guide_out ? (wout == 1 ? conv_out_kernel<1, true> : conv_out_kernel<8, true>)
+                            : (wout == 1 ? conv_out_kernel<1, false> : conv_out_kernel<8, false>);
+  TDX_CHECK_CUDA(launch(kernel, grid, 128, smem, stream, p));
   return TDX_OK;
 }
 
@@ -426,17 +416,15 @@ int embed_launch(const TdxEmbedDesc& d, cudaStream_t stream) {
   p.noise_dims = d.noise_dims;
   p.E = d.emb_channels;
   for (int b = 0; b < d.n_blocks; ++b) p.blocks[b] = d.blocks[b];
-  dim3 grid(d.n_blocks, d.n_img);
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, grid, dim3(256), 0, stream);
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, embed_kernel, p));
+  TDX_CHECK_CUDA(launch(embed_kernel, dim3(d.n_blocks, d.n_img), 256, 0, stream, p));
   return TDX_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ elementwise fp32
 __global__ void sched_step_kernel(float* sample, const float* f, float* x0_prev, int64_t n, float cs, float co, float r,
                                   float k) {
+  pdl_launch_dependents();
+  pdl_wait();
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (; i < n; i += stride) {
@@ -456,6 +444,8 @@ __device__ __forceinline__ void st4(float* p, const float4& v) { *reinterpret_ca
 template <bool VEC>
 __global__ void blend_accumulate_kernel(float* cval, float* cw, int channels, int CH, int CW, const float* tile,
                                         const float* window, int th, int tw, int y0, int x0) {
+  pdl_launch_dependents();
+  pdl_wait();
   constexpr int V = VEC ? 4 : 1;
   const int x = (blockIdx.x * blockDim.x + threadIdx.x) * V;
   const int y = blockIdx.y;
@@ -505,6 +495,8 @@ __global__ void blend_accumulate_kernel(float* cval, float* cw, int channels, in
 template <bool VEC>
 __global__ void canvas_add_kernel(float* dst, int channels, int DH, int DW, const float* tile, int th, int tw, int y0,
                                   int x0) {
+  pdl_launch_dependents();
+  pdl_wait();
   constexpr int V = VEC ? 4 : 1;
   const int x = (blockIdx.x * blockDim.x + threadIdx.x) * V;
   const int y = blockIdx.y;
@@ -535,6 +527,8 @@ __global__ void canvas_add_kernel(float* dst, int channels, int DH, int DW, cons
 template <bool VEC>
 __global__ void blend_normalize_kernel(float* out, const float* cval, const float* cw, int channels, int64_t plane,
                                        float divisor) {
+  pdl_launch_dependents();
+  pdl_wait();
   constexpr int V = VEC ? 4 : 1;
   int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * V;
   const int64_t n = plane * channels;
@@ -588,9 +582,8 @@ extern "C" int tdx_sched_step(float* sample, const float* model_out, float* x0_p
   TDX_REQUIRE(sample && model_out && x0_prev && numel > 0, "sched_step: bad arguments");
   int blocks = (int)((numel + 255) / 256);
   if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-  sched_step_kernel<<<blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(sample, model_out, x0_prev, numel,
-                                                                               c_skip, c_out, r, k);
-  TDX_CHECK_CUDA(cudaGetLastError());
+  TDX_CHECK_CUDA(launch(sched_step_kernel, blocks, 256, 0, stream, sample, model_out, x0_prev, numel, c_skip, c_out, r,
+                        k));
   return TDX_OK;
 }
 
@@ -604,15 +597,9 @@ extern "C" int tdx_blend_accumulate(float* canvas_val, float* canvas_w, int32_t 
   const bool vec = (tile_w % 4 == 0) && (canvas_w_px % 4 == 0) && (x0 % 4 == 0) && aligned16(canvas_val) &&
                    aligned16(canvas_w) && aligned16(tile) && aligned16(window) &&
                    ((size_t)canvas_h * canvas_w_px) % 4 == 0 && ((size_t)tile_h * tile_w) % 4 == 0;
-  if (vec) {
-    grid.x = (tile_w / 4 + 127) / 128;
-    blend_accumulate_kernel<true><<<grid, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        canvas_val, canvas_w, channels, canvas_h, canvas_w_px, tile, window, tile_h, tile_w, y0, x0);
-  } else {
-    blend_accumulate_kernel<false><<<grid, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        canvas_val, canvas_w, channels, canvas_h, canvas_w_px, tile, window, tile_h, tile_w, y0, x0);
-  }
-  TDX_CHECK_CUDA(cudaGetLastError());
+  if (vec) grid.x = (tile_w / 4 + 127) / 128;
+  TDX_CHECK_CUDA(launch(vec ? blend_accumulate_kernel<true> : blend_accumulate_kernel<false>, grid, 128, 0, stream,
+                        canvas_val, canvas_w, channels, canvas_h, canvas_w_px, tile, window, tile_h, tile_w, y0, x0));
   return TDX_OK;
 }
 
@@ -623,15 +610,9 @@ extern "C" int tdx_canvas_add(float* dst, int32_t channels, int32_t dst_h, int32
   dim3 grid((tile_w + 127) / 128, tile_h);
   const bool vec = (tile_w % 4 == 0) && (dst_w % 4 == 0) && (x0 % 4 == 0) && aligned16(dst) && aligned16(tile) &&
                    ((size_t)dst_h * dst_w) % 4 == 0 && ((size_t)tile_h * tile_w) % 4 == 0;
-  if (vec) {
-    grid.x = (tile_w / 4 + 127) / 128;
-    canvas_add_kernel<true><<<grid, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(dst, channels, dst_h, dst_w, tile,
-                                                                                     tile_h, tile_w, y0, x0);
-  } else {
-    canvas_add_kernel<false><<<grid, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(dst, channels, dst_h, dst_w, tile,
-                                                                                      tile_h, tile_w, y0, x0);
-  }
-  TDX_CHECK_CUDA(cudaGetLastError());
+  if (vec) grid.x = (tile_w / 4 + 127) / 128;
+  TDX_CHECK_CUDA(launch(vec ? canvas_add_kernel<true> : canvas_add_kernel<false>, grid, 128, 0, stream, dst, channels,
+                        dst_h, dst_w, tile, tile_h, tile_w, y0, x0));
   return TDX_OK;
 }
 
@@ -643,12 +624,7 @@ extern "C" int tdx_blend_normalize(float* out, const float* canvas_val, const fl
   int blocks = (int)((n / (vec ? 4 : 1) + 255) / 256);
   if (blocks > sm_count() * 8) blocks = sm_count() * 8;
   if (blocks < 1) blocks = 1;
-  if (vec)
-    blend_normalize_kernel<true><<<blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(out, canvas_val, canvas_w,
-                                                                                            channels, plane, divisor);
-  else
-    blend_normalize_kernel<false><<<blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(out, canvas_val, canvas_w,
-                                                                                             channels, plane, divisor);
-  TDX_CHECK_CUDA(cudaGetLastError());
+  TDX_CHECK_CUDA(launch(vec ? blend_normalize_kernel<true> : blend_normalize_kernel<false>, blocks, 256, 0, stream, out,
+                        canvas_val, canvas_w, channels, plane, divisor));
   return TDX_OK;
 }

@@ -94,16 +94,6 @@ __global__ void detail_raw_kernel(const float* __restrict__ elev, const float* _
   }
 }
 
-template <typename Kernel, typename... Args>
-int launch_flat(Kernel kernel, long n, void* stream, Args... args) {   // one thread per element, 256 per block
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3((unsigned)((n + 255) / 256)), dim3(256), 0,
-                     reinterpret_cast<cudaStream_t>(stream));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, args...));
-  return TDX_OK;
-}
-
 }  // namespace tdx
 
 using namespace tdx;
@@ -115,10 +105,7 @@ extern "C" int tdx_detail_range(const float* x, int64_t n, uint32_t* range, void
   TDX_CHECK_CUDA(cudaMemsetAsync(range, 0, 2 * sizeof(uint32_t), st));
   const long blocks = (n + 255) / 256;
   const int grid = (int)(blocks < 4L * sm_count() ? blocks : 4L * sm_count());
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3(grid), dim3(256), 0, st);
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, detail_range_kernel, x, (long)n, reinterpret_cast<unsigned*>(range)));
+  TDX_CHECK_CUDA(launch(detail_range_kernel, grid, 256, 0, st, x, (long)n, reinterpret_cast<unsigned*>(range)));
   return TDX_OK;
 }
 
@@ -127,20 +114,25 @@ extern "C" int tdx_detail_colour(const float* x, int64_t n, const uint32_t* rang
   TDX_REQUIRE(x && range && lut && out, "detail_colour: null pointer");
   TDX_REQUIRE(n >= 1, "detail_colour: empty input");
   TDX_REQUIRE(reinterpret_cast<uintptr_t>(out) % 4 == 0, "detail_colour: out must be 4-byte aligned");
-  return launch_flat(detail_colour_kernel, (long)n, stream, x, (long)n, reinterpret_cast<const unsigned*>(range), lut,
-                     reinterpret_cast<uchar4*>(out));
+  TDX_CHECK_CUDA(launch(detail_colour_kernel, (unsigned)((n + 255) / 256), 256, 0, stream, x, (long)n,
+                        reinterpret_cast<const unsigned*>(range), lut, reinterpret_cast<uchar4*>(out)));
+  return TDX_OK;
 }
 
 extern "C" int tdx_detail_rgba8(const float* rgb, int64_t n, uint8_t* out, void* stream) {
   TDX_REQUIRE(rgb && out, "detail_rgba8: null pointer");
   TDX_REQUIRE(n >= 1, "detail_rgba8: empty input");
   TDX_REQUIRE(reinterpret_cast<uintptr_t>(out) % 4 == 0, "detail_rgba8: out must be 4-byte aligned");
-  return launch_flat(detail_rgba8_kernel, (long)n, stream, rgb, (long)n, reinterpret_cast<uchar4*>(out));
+  TDX_CHECK_CUDA(launch(detail_rgba8_kernel, (unsigned)((n + 255) / 256), 256, 0, stream, rgb, (long)n,
+                        reinterpret_cast<uchar4*>(out)));
+  return TDX_OK;
 }
 
 extern "C" int tdx_detail_raw(const float* elev, const float* temp, int64_t n, void* body, void* stream) {
   TDX_REQUIRE(elev && body, "detail_raw: null pointer");
   TDX_REQUIRE(n >= 1, "detail_raw: empty input");
   TDX_REQUIRE(reinterpret_cast<uintptr_t>(body) % 2 == 0, "detail_raw: body must be 2-byte aligned");
-  return launch_flat(detail_raw_kernel, (long)n, stream, elev, temp, (long)n, static_cast<uint16_t*>(body));
+  TDX_CHECK_CUDA(launch(detail_raw_kernel, (unsigned)((n + 255) / 256), 256, 0, stream, elev, temp, (long)n,
+                        static_cast<uint16_t*>(body)));
+  return TDX_OK;
 }

@@ -237,10 +237,7 @@ extern "C" int tdx_flow_d8(const float* z, int32_t h, int32_t w, float tol, int8
   q.tiles_x = (w + kFlowTileW - 1) / kFlowTileW;
   q.kmax = kmax; q.is_sink = is_sink; q.rr = rr; q.cc = cc; q.recv = recv; q.indeg = indeg; q.flags = flags;
   const long tiles = (long)q.tiles_x * ((h + kFlowTileH - 1) / kFlowTileH);
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3((unsigned)tiles), dim3(kFlowTileW * kFlowTileH), 0, st);
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, flow_d8_kernel, q));
+  TDX_CHECK_CUDA(launch(flow_d8_kernel, (unsigned)tiles, kFlowTileW * kFlowTileH, 0, st, q));
   return TDX_OK;
 }
 
@@ -253,10 +250,8 @@ extern "C" int tdx_flow_link(const float* z, const int64_t* rr, const int64_t* c
   const long n = (long)h * w;
   TDX_CHECK_CUDA(cudaMemsetAsync(flags, 0, sizeof(uint32_t), st));
   TDX_CHECK_CUDA(cudaMemsetAsync(indeg, 0, n * sizeof(uint32_t), st));
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st);
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, flow_link_kernel, z, rr, cc, is_sink, (int)h, (int)w, recv, indeg, flags));
+  TDX_CHECK_CUDA(launch(flow_link_kernel, (unsigned)((n + 255) / 256), 256, 0, st, z, rr, cc, is_sink, (int)h, (int)w,
+                        recv, indeg, flags));
   return TDX_OK;
 }
 
@@ -266,11 +261,8 @@ extern "C" int tdx_flow_accumulate(const float* z, int64_t n, const int32_t* rec
   TDX_REQUIRE(n >= 1 && n <= kFlowMaxPixels, "flow_accumulate: %lld px (1 .. 2^24)", (long long)n);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   TDX_CHECK_CUDA(cudaMemsetAsync(state, 0, n * sizeof(uint64_t), st));
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st);
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, flow_accumulate_kernel, z, recv, indeg,
-                                    reinterpret_cast<unsigned long long*>(state), A, (int)n));
+  TDX_CHECK_CUDA(launch(flow_accumulate_kernel, (unsigned)((n + 255) / 256), 256, 0, st, z, recv, indeg,
+                        reinterpret_cast<unsigned long long*>(state), A, (int)n));
   return TDX_OK;
 }
 
@@ -281,10 +273,7 @@ extern "C" int tdx_flow_indicator(const float* A, int32_t h, int32_t w, int32_t 
   if (oh == 0 || ow == 0) return TDX_OK;   // k exceeds the image: an empty result
   TDX_REQUIRE(A && out, "flow_indicator: null pointer");
   const long m = (long)oh * ow;
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3((unsigned)((m + 255) / 256)), dim3(256), 0,
-                     reinterpret_cast<cudaStream_t>(stream));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, flow_indicator_kernel, A, (int)w, (int)k, oh, ow, out));
+  TDX_CHECK_CUDA(launch(flow_indicator_kernel, (unsigned)((m + 255) / 256), 256, 0, stream, A, (int)w, (int)k, oh, ow,
+                        out));
   return TDX_OK;
 }

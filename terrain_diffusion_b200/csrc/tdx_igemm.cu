@@ -1035,18 +1035,8 @@ int igemm_launch(const TdxIgemmDesc& d, const CUtensorMap* tms, cudaStream_t str
   const CUtensorMap& t0 = tms[0];
   const CUtensorMap& t1 = tms[d.n_seg > 1 ? 1 : 0];
   const CUtensorMap& t2 = tms[d.n_seg > 2 ? 2 : 0];
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[2];
-  fill_launch_config(&cfg, attr, dim3(grid), dim3(kThreads), smem < 120 * 1024 ? 120 * 1024 : smem, stream);
-  if (cluster > 1) {
-    attr[cfg.numAttrs].id = cudaLaunchAttributeClusterDimension;
-    attr[cfg.numAttrs].val.clusterDim.x = cluster;
-    attr[cfg.numAttrs].val.clusterDim.y = 1;
-    attr[cfg.numAttrs].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs += 1;
-  }
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, igemm_kernel_for(cluster > 1, p.ncta), t0, t1, t2, p));
+  TDX_CHECK_CUDA(launch_clustered(cluster, igemm_kernel_for(cluster > 1, p.ncta), grid, kThreads,
+                                  smem < 120 * 1024 ? 120 * 1024 : smem, stream, t0, t1, t2, p));
   return TDX_OK;
 }
 

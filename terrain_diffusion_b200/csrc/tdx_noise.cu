@@ -12,6 +12,7 @@
 // the requested patch -- at their exact stream positions.  Acceptance uses the reference's fp64 arithmetic with
 // separately rounded multiplies and adds (no FMA contraction), so the integer stream positions are bit-exact.
 #include "tdx_common.h"
+#include "tdx_ptx.cuh"
 
 namespace tdx {
 
@@ -51,8 +52,8 @@ __device__ __forceinline__ bool polar_pair(unsigned long long& state, double& v1
   return s > 0.0 && s < 1.0;
 }
 
-__global__ void noise_count_kernel(unsigned long long seed, long long n_pairs, int* counts) {
-  const long long chunk = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+// Pass 1: how many of the candidate pairs of `chunk` the polar method accepts.
+__device__ __forceinline__ void count_chunk(unsigned long long seed, long long n_pairs, long long chunk, int* counts) {
   const long long p0 = chunk * kChunk;
   if (p0 >= n_pairs) return;
   unsigned long long state = lcg_jump(seed, 2ULL * (unsigned long long)p0);
@@ -64,8 +65,8 @@ __global__ void noise_count_kernel(unsigned long long seed, long long n_pairs, i
   counts[chunk] = c;
 }
 
-// Exclusive scan of `n` ints in place, single block (n is a few tens of thousands at most).
-__global__ void noise_scan_kernel(int* counts, long long n) {
+// Pass 2: exclusive scan of `n` ints in place by one block (n is a few tens of thousands at most).
+__device__ __forceinline__ void scan_counts(int* counts, long long n) {
   __shared__ int warp_tot[32];
   __shared__ int carry;
   if (threadIdx.x == 0) carry = 0;
@@ -122,14 +123,13 @@ __device__ __forceinline__ void noise_store(const NoiseEmit& p, long long idx, d
   p.out[((long long)c * p.h + (Y - p.y0)) * p.w + (X - p.x0)] = (float)val;
 }
 
-__global__ void noise_emit_kernel(const NoiseEmit p, const int* offsets, long long n_chunks) {
-  const long long chunk = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+// Pass 3: regenerate the pairs of `chunk` and store the normals that fall inside the patch at their stream positions.
+// The last chunk flags a budget that ran out before the stream was complete.
+__device__ __forceinline__ void emit_chunk(const NoiseEmit& p, const int* offsets, long long chunk,
+                                           long long n_chunks) {
   if (chunk >= n_chunks) return;
   const long long p0 = chunk * kChunk;
   long long pos = 2LL * offsets[chunk];
-  if (chunk == n_chunks - 1) {
-    // last chunk: the budget must cover the whole stream
-  }
   if (pos >= p.n_out) return;
   unsigned long long state = lcg_jump(p.seed, 2ULL * (unsigned long long)p0);
   for (int i = 0; i < kChunk && p0 + i < p.n_pairs; ++i) {
@@ -145,6 +145,25 @@ __global__ void noise_emit_kernel(const NoiseEmit p, const int* offsets, long lo
   if (chunk == n_chunks - 1 && pos < p.n_out) *p.status = 1;
 }
 
+// ---- single form: one (patch, tile) job per launch
+__global__ void noise_count_kernel(unsigned long long seed, long long n_pairs, int* counts) {
+  pdl_launch_dependents();
+  pdl_wait();
+  count_chunk(seed, n_pairs, (long long)blockIdx.x * blockDim.x + threadIdx.x, counts);
+}
+
+__global__ void noise_scan_kernel(int* counts, long long n_chunks) {
+  pdl_launch_dependents();
+  pdl_wait();
+  scan_counts(counts, n_chunks);
+}
+
+__global__ void noise_emit_kernel(const NoiseEmit p, const int* offsets, long long n_chunks) {
+  pdl_launch_dependents();
+  pdl_wait();
+  emit_chunk(p, offsets, (long long)blockIdx.x * blockDim.x + threadIdx.x, n_chunks);
+}
+
 // ---- batched form: up to kBatchJobs (patch, tile) jobs per launch, job = blockIdx.y, one counts slice per job
 constexpr int kBatchJobs = 32;
 struct NoiseBatch {
@@ -154,79 +173,24 @@ struct NoiseBatch {
 };
 
 __global__ void noise_count_batch_kernel(const __grid_constant__ NoiseBatch b, int* counts) {
+  pdl_launch_dependents();
+  pdl_wait();
   const NoiseEmit& p = b.job[blockIdx.y];
-  const long long chunk = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const long long p0 = chunk * kChunk;
-  if (p0 >= p.n_pairs) return;
-  unsigned long long state = lcg_jump(p.seed, 2ULL * (unsigned long long)p0);
-  int c = 0;
-  for (int i = 0; i < kChunk && p0 + i < p.n_pairs; ++i) {
-    double v1, v2, s;
-    c += polar_pair(state, v1, v2, s) ? 1 : 0;
-  }
-  counts[(long long)blockIdx.y * b.n_chunks + chunk] = c;
-}
-
-__device__ __forceinline__ void scan_block(int* counts, long long n) {
-  __shared__ int warp_tot[32];
-  __shared__ int carry;
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (long long base = 0; base < n; base += blockDim.x) {
-    const long long i = base + threadIdx.x;
-    const int v = i < n ? counts[i] : 0;
-    int incl = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int t = __shfl_up_sync(0xffffffff, incl, o);
-      if (lane >= o) incl += t;
-    }
-    if (lane == 31) warp_tot[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-      int w = lane < (int)(blockDim.x >> 5) ? warp_tot[lane] : 0;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int t = __shfl_up_sync(0xffffffff, w, o);
-        if (lane >= o) w += t;
-      }
-      warp_tot[lane] = w;
-    }
-    __syncthreads();
-    const int warp_off = warp == 0 ? 0 : warp_tot[warp - 1];
-    const int block_total = warp_tot[(blockDim.x >> 5) - 1];
-    if (i < n) counts[i] = carry + warp_off + incl - v;
-    __syncthreads();
-    if (threadIdx.x == 0) carry += block_total;
-    __syncthreads();
-  }
+  count_chunk(p.seed, p.n_pairs, (long long)blockIdx.x * blockDim.x + threadIdx.x,
+              counts + (long long)blockIdx.y * b.n_chunks);
 }
 
 __global__ void noise_scan_batch_kernel(int* counts, long long n_chunks) {
-  scan_block(counts + (long long)blockIdx.x * n_chunks, n_chunks);
+  pdl_launch_dependents();
+  pdl_wait();
+  scan_counts(counts + (long long)blockIdx.x * n_chunks, n_chunks);
 }
 
 __global__ void noise_emit_batch_kernel(const __grid_constant__ NoiseBatch b, const int* counts) {
-  const NoiseEmit& p = b.job[blockIdx.y];
-  const int* offsets = counts + (long long)blockIdx.y * b.n_chunks;
-  const long long chunk = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (chunk >= b.n_chunks) return;
-  const long long p0 = chunk * kChunk;
-  long long pos = 2LL * offsets[chunk];
-  if (pos >= p.n_out) return;
-  unsigned long long state = lcg_jump(p.seed, 2ULL * (unsigned long long)p0);
-  for (int i = 0; i < kChunk && p0 + i < p.n_pairs; ++i) {
-    double v1, v2, s;
-    if (polar_pair(state, v1, v2, s)) {
-      const double f = sqrt(__ddiv_rn(__dmul_rn(-2.0, log(s)), s));
-      noise_store(p, pos, __dmul_rn(v1, f));
-      noise_store(p, pos + 1, __dmul_rn(v2, f));
-      pos += 2;
-      if (pos >= p.n_out) return;
-    }
-  }
-  if (chunk == b.n_chunks - 1 && pos < p.n_out) *p.status = 1;
+  pdl_launch_dependents();
+  pdl_wait();
+  emit_chunk(b.job[blockIdx.y], counts + (long long)blockIdx.y * b.n_chunks,
+             (long long)blockIdx.x * blockDim.x + threadIdx.x, b.n_chunks);
 }
 
 static long long floordiv(long long a, long long b) {
@@ -246,6 +210,17 @@ unsigned long long tile_seed(unsigned long long base, long long ty, long long tx
   h = h + ((unsigned long long)ty & 0xFFFFFFFFULL);
   h = h * 0x9E3779B9ULL + ((unsigned long long)tx & 0xFFFFFFFFULL);
   return h;
+}
+
+constexpr int kNoiseThreads = 128;   // threads of the count and emit passes; the scan runs on one 1024-thread block
+
+// The three passes of one single-form job, counts[n_chunks] as their scratch.
+static int run_noise_job(const NoiseEmit& p, int* counts, long long n_chunks, cudaStream_t stream) {
+  const int blocks = (int)((n_chunks + kNoiseThreads - 1) / kNoiseThreads);
+  TDX_CHECK_CUDA(launch(noise_count_kernel, blocks, kNoiseThreads, 0, stream, p.seed, p.n_pairs, counts));
+  TDX_CHECK_CUDA(launch(noise_scan_kernel, 1, 1024, 0, stream, counts, n_chunks));
+  TDX_CHECK_CUDA(launch(noise_emit_kernel, blocks, kNoiseThreads, 0, stream, p, counts, n_chunks));
+  return TDX_OK;
 }
 
 }  // namespace tdx
@@ -277,31 +252,14 @@ extern "C" int tdx_noise_patch(uint64_t base_seed, int64_t y0, int64_t x0, int32
   TDX_CHECK_CUDA(cudaMemsetAsync(status, 0, sizeof(int), stream));
   const long long ty0 = floordiv(y0, tile_h), ty1 = floordiv(y0 + h - 1, tile_h);
   const long long tx0 = floordiv(x0, tile_w), tx1 = floordiv(x0 + w - 1, tile_w);
-  const int threads = 128;
-  const int blocks = (int)((n_chunks + threads - 1) / threads);
   for (long long ty = ty0; ty <= ty1; ++ty) {
     for (long long tx = tx0; tx <= tx1; ++tx) {
-      NoiseEmit p;
-      p.seed = tile_seed(base_seed, ty, tx);
-      p.n_pairs = n_pairs;
-      p.n_out = n_out;
-      p.tile_h = tile_h;
-      p.tile_w = tile_w;
-      p.tile_y0 = ty * tile_h;
-      p.tile_x0 = tx * tile_w;
-      p.y0 = y0;
-      p.x0 = x0;
-      p.h = h;
-      p.w = w;
-      p.channels = channels;
-      p.out = out;
-      p.status = status;
-      noise_count_kernel<<<blocks, threads, 0, stream>>>(p.seed, n_pairs, counts);
-      noise_scan_kernel<<<1, 1024, 0, stream>>>(counts, n_chunks);
-      noise_emit_kernel<<<blocks, threads, 0, stream>>>(p, counts, n_chunks);
+      const NoiseEmit p = {tile_seed(base_seed, ty, tx), n_pairs, n_out, tile_h, tile_w, ty * tile_h, tx * tile_w, y0,
+                           x0, h, w, channels, out, status};
+      int rc = run_noise_job(p, counts, n_chunks, stream);
+      if (rc != TDX_OK) return rc;
     }
   }
-  TDX_CHECK_CUDA(cudaGetLastError());
   return TDX_OK;
 }
 
@@ -330,17 +288,15 @@ extern "C" int tdx_noise_patches(uint64_t base_seed, int32_t n_patches, const in
   int* status = reinterpret_cast<int*>(workspace);
   int* counts = status + 64;
   TDX_CHECK_CUDA(cudaMemsetAsync(status, 0, sizeof(int), stream));
-  const int threads = 128;
-  const int blocks = (int)((n_chunks + threads - 1) / threads);
+  const int blocks = (int)((n_chunks + kNoiseThreads - 1) / kNoiseThreads);
   NoiseBatch b;
   b.n_jobs = 0;
   b.n_chunks = n_chunks;
   auto flush = [&]() -> int {
     if (b.n_jobs == 0) return TDX_OK;
-    noise_count_batch_kernel<<<dim3(blocks, b.n_jobs), threads, 0, stream>>>(b, counts);
-    noise_scan_batch_kernel<<<b.n_jobs, 1024, 0, stream>>>(counts, n_chunks);
-    noise_emit_batch_kernel<<<dim3(blocks, b.n_jobs), threads, 0, stream>>>(b, counts);
-    TDX_CHECK_CUDA(cudaGetLastError());
+    TDX_CHECK_CUDA(launch(noise_count_batch_kernel, dim3(blocks, b.n_jobs), kNoiseThreads, 0, stream, b, counts));
+    TDX_CHECK_CUDA(launch(noise_scan_batch_kernel, b.n_jobs, 1024, 0, stream, counts, n_chunks));
+    TDX_CHECK_CUDA(launch(noise_emit_batch_kernel, dim3(blocks, b.n_jobs), kNoiseThreads, 0, stream, b, counts));
     b.n_jobs = 0;
     return TDX_OK;
   };
@@ -350,21 +306,8 @@ extern "C" int tdx_noise_patches(uint64_t base_seed, int32_t n_patches, const in
     const long long tx0 = floordiv(x0, tile_w), tx1 = floordiv(x0 + w - 1, tile_w);
     for (long long ty = ty0; ty <= ty1; ++ty) {
       for (long long tx = tx0; tx <= tx1; ++tx) {
-        NoiseEmit& p = b.job[b.n_jobs++];
-        p.seed = tile_seed(base_seed, ty, tx);
-        p.n_pairs = n_pairs;
-        p.n_out = n_out;
-        p.tile_h = tile_h;
-        p.tile_w = tile_w;
-        p.tile_y0 = ty * tile_h;
-        p.tile_x0 = tx * tile_w;
-        p.y0 = y0;
-        p.x0 = x0;
-        p.h = h;
-        p.w = w;
-        p.channels = channels;
-        p.out = out + (long long)i * channels * h * w;
-        p.status = status;
+        b.job[b.n_jobs++] = {tile_seed(base_seed, ty, tx), n_pairs, n_out, tile_h, tile_w, ty * tile_h, tx * tile_w,
+                             y0, x0, h, w, channels, out + (long long)i * channels * h * w, status};
         if (b.n_jobs == kBatchJobs) {
           int rc = flush();
           if (rc != TDX_OK) return rc;
@@ -388,28 +331,8 @@ extern "C" int tdx_standard_normal(uint64_t seed, int64_t n, float* out, void* w
   int* status = reinterpret_cast<int*>(workspace);
   int* counts = status + 64;
   TDX_CHECK_CUDA(cudaMemsetAsync(status, 0, sizeof(int), stream));
-  NoiseEmit p;
-  p.seed = seed;
-  p.n_pairs = n_pairs;
-  p.n_out = n;
-  p.tile_h = 1;
-  p.tile_w = (int)n;
-  p.tile_y0 = 0;
-  p.tile_x0 = 0;
-  p.y0 = 0;
-  p.x0 = 0;
-  p.h = 1;
-  p.w = (int)n;
-  p.channels = 1;
-  p.out = out;
-  p.status = status;
-  const int threads = 128;
-  const int blocks = (int)((n_chunks + threads - 1) / threads);
-  noise_count_kernel<<<blocks, threads, 0, stream>>>(p.seed, n_pairs, counts);
-  noise_scan_kernel<<<1, 1024, 0, stream>>>(counts, n_chunks);
-  noise_emit_kernel<<<blocks, threads, 0, stream>>>(p, counts, n_chunks);
-  TDX_CHECK_CUDA(cudaGetLastError());
-  return TDX_OK;
+  const NoiseEmit p = {seed, n_pairs, n, 1, (int)n, 0, 0, 0, 0, 1, (int)n, 1, out, status};
+  return run_noise_job(p, counts, n_chunks, stream);
 }
 
 /* Reads back the overflow flag written by the last tdx_noise_patch on this workspace (synchronises the stream). */

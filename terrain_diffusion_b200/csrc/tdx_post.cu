@@ -266,11 +266,6 @@ __global__ void climate_sample_kernel(const ClimateParams p) {
   p.out[4 * plane + o] = be;
 }
 
-static int launch2d(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, int h, int w, cudaStream_t stream) {
-  fill_launch_config(cfg, attr, dim3((w + 127) / 128, h), dim3(128), 0, stream);
-  return TDX_OK;
-}
-
 }  // namespace tdx
 
 using namespace tdx;
@@ -280,21 +275,16 @@ extern "C" int tdx_post_normalize(const float* num, const float* den, int64_t pi
   TDX_REQUIRE(num && den && out, "post_normalize: null pointer");
   TDX_REQUIRE(h >= 1 && w >= 1 && h <= 65535 && pitch >= w, "post_normalize: bad shape %d x %d (pitch %lld)", h, w,
               (long long)pitch);
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  launch2d(&cfg, attr, h, w, reinterpret_cast<cudaStream_t>(stream));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, post_normalize_kernel, num, den, (long)pitch, out, (int)h, (int)w, scale,
-                                    offset));
+  TDX_CHECK_CUDA(launch(post_normalize_kernel, dim3((w + 127) / 128, h), 128, 0, stream, num, den, (long)pitch, out,
+                        (int)h, (int)w, scale, offset));
   return TDX_OK;
 }
 
 extern "C" int tdx_post_pad_extrapolate(const float* x, int32_t h, int32_t w, float* out, void* stream) {
   TDX_REQUIRE(x && out, "post_pad_extrapolate: null pointer");
   TDX_REQUIRE(h >= 1 && w >= 1 && h + 2 <= 65535, "post_pad_extrapolate: bad shape %d x %d", h, w);
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  launch2d(&cfg, attr, h + 2, w + 2, reinterpret_cast<cudaStream_t>(stream));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, post_pad_extrapolate_kernel, x, (int)h, (int)w, out));
+  TDX_CHECK_CUDA(launch(post_pad_extrapolate_kernel, dim3((w + 2 + 127) / 128, h + 2), 128, 0, stream, x, (int)h,
+                        (int)w, out));
   return TDX_OK;
 }
 
@@ -305,10 +295,8 @@ extern "C" int tdx_resize_aa_axis(const float* x, int32_t h, int32_t w, float* o
   TDX_REQUIRE(h >= 1 && w >= 1 && out_size >= 1, "resize_aa_axis: bad shape %d x %d -> %d", h, w, out_size);
   const int oh = axis == 0 ? out_size : h, ow = axis == 1 ? out_size : w;
   TDX_REQUIRE(oh <= 65535, "resize_aa_axis: more than 65535 output rows");
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  launch2d(&cfg, attr, oh, ow, reinterpret_cast<cudaStream_t>(stream));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, resize_aa_axis_kernel, x, (int)h, (int)w, out, (int)out_size, (int)axis));
+  TDX_CHECK_CUDA(launch(resize_aa_axis_kernel, dim3((ow + 127) / 128, oh), 128, 0, stream, x, (int)h, (int)w, out,
+                        (int)out_size, (int)axis));
   return TDX_OK;
 }
 
@@ -330,10 +318,7 @@ extern "C" int tdx_gaussian_blur(const float* x, int32_t h, int32_t w, float* ou
     sum += bp.k[i];
   }
   for (int i = 0; i < ksize; ++i) bp.k[i] /= sum;
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  launch2d(&cfg, attr, h, w, reinterpret_cast<cudaStream_t>(stream));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gaussian_blur_kernel, x, (int)h, (int)w, out, bp));
+  TDX_CHECK_CUDA(launch(gaussian_blur_kernel, dim3((w + 127) / 128, h), 128, 0, stream, x, (int)h, (int)w, out, bp));
   return TDX_OK;
 }
 
@@ -341,11 +326,8 @@ extern "C" int tdx_post_combine(const float* a, int64_t a_pitch, const float* b,
                                 int16_t* out_i16, int32_t h, int32_t w, int32_t signed_square, void* stream) {
   TDX_REQUIRE(a && b && (out || out_i16), "post_combine: null pointer");
   TDX_REQUIRE(h >= 1 && w >= 1 && h <= 65535 && a_pitch >= w && b_pitch >= w, "post_combine: bad shape %d x %d", h, w);
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  launch2d(&cfg, attr, h, w, reinterpret_cast<cudaStream_t>(stream));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, post_combine_kernel, a, (long)a_pitch, b, (long)b_pitch, out, out_i16, (int)h,
-                                    (int)w, (int)signed_square));
+  TDX_CHECK_CUDA(launch(post_combine_kernel, dim3((w + 127) / 128, h), 128, 0, stream, a, (long)a_pitch, b,
+                        (long)b_pitch, out, out_i16, (int)h, (int)w, (int)signed_square));
   return TDX_OK;
 }
 
@@ -366,10 +348,7 @@ extern "C" int tdx_terrain_upsample(const float* elev, const float* climate, int
   p.h = h; p.w = w; p.scale = scale; p.oi = oi; p.oj = oj; p.H = H; p.W = W;
   p.small = ((int64_t)h + w) * scale <= 128;
   p.r = (float)(1.0 / scale);                          // compute_scales_value: static_cast<float>(1.0 / scale)
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  launch2d(&cfg, attr, H, W, reinterpret_cast<cudaStream_t>(stream));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, terrain_upsample_kernel, p));
+  TDX_CHECK_CUDA(launch(terrain_upsample_kernel, dim3((W + 127) / 128, H), 128, 0, stream, p));
   return TDX_OK;
 }
 
@@ -383,10 +362,8 @@ extern "C" int tdx_lapse_rate(const float* temp, const float* coarse_elev_sqrt, 
   p.h = h; p.w = w; p.win = win;
   p.beta_lo = beta_lo; p.beta_hi = beta_hi; p.fallback_beta = fallback_beta; p.eps = eps;
   p.fallback_threshold = fallback_threshold;
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  launch2d(&cfg, attr, h - win + 1, w - win + 1, reinterpret_cast<cudaStream_t>(stream));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, lapse_rate_kernel, temp, coarse_elev_sqrt, t_sea, beta, p));
+  TDX_CHECK_CUDA(launch(lapse_rate_kernel, dim3((w - win + 1 + 127) / 128, h - win + 1), 128, 0, stream, temp,
+                        coarse_elev_sqrt, t_sea, beta, p));
   return TDX_OK;
 }
 
@@ -402,9 +379,6 @@ extern "C" int tdx_climate_sample(const float* t_sea, const float* beta, const f
   p.t_sea = t_sea; p.beta = beta; p.coarse = coarse; p.elev = elev; p.out = out;
   p.hc = hc; p.wc = wc; p.crop = crop; p.hs = hc - 2 * crop; p.ws = wc - 2 * crop;
   p.i1 = i1; p.j1 = j1; p.h = h; p.w = w; p.S = coarse_stride; p.ci1 = ci1; p.cj1 = cj1;
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  launch2d(&cfg, attr, h, w, reinterpret_cast<cudaStream_t>(stream));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, climate_sample_kernel, p));
+  TDX_CHECK_CUDA(launch(climate_sample_kernel, dim3((w + 127) / 128, h), 128, 0, stream, p));
   return TDX_OK;
 }

@@ -193,10 +193,7 @@ extern "C" int tdx_relief_stats(const float* elev, int64_t n, uint32_t* stats, v
   TDX_CHECK_CUDA(cudaMemsetAsync(stats, 0, 3 * sizeof(uint32_t), st));
   const long blocks = (n + 255) / 256;
   const int grid = (int)(blocks < 4L * sm_count() ? blocks : 4L * sm_count());
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3(grid), dim3(256), 0, st);
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, relief_stats_kernel, elev, (long)n, reinterpret_cast<unsigned*>(stats)));
+  TDX_CHECK_CUDA(launch(relief_stats_kernel, grid, 256, 0, st, elev, (long)n, reinterpret_cast<unsigned*>(stats)));
   return TDX_OK;
 }
 
@@ -221,13 +218,11 @@ extern "C" int tdx_relief_gaussian(const float* x, int32_t h, int32_t w, int32_t
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long plane = (long)h * w;
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3((w + 127) / 128, h, n_sigma), dim3(128), 0, st);
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, relief_gauss_kernel, x, 0L, tmp, (int)h, (int)w, 0, (int)replace_nan,
-                                    nan_fill, t));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, relief_gauss_kernel, (const float*)tmp, plane, out, (int)h, (int)w, 1, 0,
-                                    0.f, t));
+  const dim3 grid((w + 127) / 128, h, n_sigma);
+  TDX_CHECK_CUDA(launch(relief_gauss_kernel, grid, 128, 0, st, x, 0L, tmp, (int)h, (int)w, 0, (int)replace_nan,
+                        nan_fill, t));
+  TDX_CHECK_CUDA(launch(relief_gauss_kernel, grid, 128, 0, st, (const float*)tmp, plane, out, (int)h, (int)w, 1, 0,
+                        0.f, t));
   return TDX_OK;
 }
 
@@ -246,9 +241,6 @@ extern "C" int tdx_relief_shade(const float* elev, const float* blurred, const u
   q.nan_fill = nan_fill; q.grad_div = grad_div; q.relief = relief; q.one_minus_relief = one_minus_relief;
   q.vmin = vmin; q.denom = denom;
   q.az = az_rad; q.sin_alt = sin_alt; q.cos_alt = cos_alt;
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3((w + 127) / 128, h), dim3(128), 0, reinterpret_cast<cudaStream_t>(stream));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, relief_shade_kernel, q));
+  TDX_CHECK_CUDA(launch(relief_shade_kernel, dim3((w + 127) / 128, h), 128, 0, stream, q));
   return TDX_OK;
 }

@@ -2,11 +2,14 @@
 // what the reference does with a dozen small torch ops per tile around the U-Net
 // (inference/world_pipeline.py:1097-1098,1128-1131,1223-1226,1235-1242).
 #include "tdx_common.h"
+#include "tdx_ptx.cuh"
 
 namespace tdx {
 
 // x_t = a * sample + b * noise   (TrigFlow re-noising: a = cos t, b = sin t * sigma_data; sample == nullptr: 0)
 __global__ void trig_mix_kernel(float* out, const float* sample, const float* noise, int64_t n, float a, float b) {
+  pdl_launch_dependents();
+  pdl_wait();
   int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x * 4;
   for (; i + 3 < n; i += stride) {
@@ -23,6 +26,8 @@ __global__ void trig_mix_kernel(float* out, const float* sample, const float* no
 // out[img][c] = x[img][c] * scale * w ; out[img][C] = w        (packed window output cat([x*w, w]))
 __global__ void pack_weighted_kernel(float* out, const float* x, const float* w, int channels, int64_t plane,
                                      float scale) {
+  pdl_launch_dependents();
+  pdl_wait();
   const int img = blockIdx.y;
   const float* xi = x + (size_t)img * channels * plane;
   float* oi = out + (size_t)img * (channels + 1) * plane;
@@ -45,6 +50,8 @@ __global__ void pack_weighted_kernel(float* out, const float* x, const float* w,
 // cond[img][c][Y][X] = packed[img][c][Y/f][X/f] / packed[img][last][Y/f][X/f]   for c < keep: normalise-on-read of a
 // packed (sum x*w, sum w) window + nearest-neighbour upsampling by f, one pass
 __global__ void window_to_cond_kernel(float* out, const float* packed, int packed_ch, int keep, int h, int w, int f) {
+  pdl_launch_dependents();
+  pdl_wait();
   const int img = blockIdx.z, c = blockIdx.y;
   const int H = h * f, W = w * f;
   const float* pv = packed + ((size_t)img * packed_ch + c) * h * w;
@@ -76,6 +83,8 @@ __device__ __forceinline__ float coarse_denorm(float x, float sigma_data, float 
 __global__ void __launch_bounds__(COARSE_EPI_THREADS)
 coarse_epilogue_kernel(float* out, const float* x, const float* means, const float* stds, const float* w, int size,
                        int pool, int elev_mode, int p5_mode, float sigma_data) {
+  pdl_launch_dependents();
+  pdl_wait();
   __shared__ float v[COARSE_EPI_MAX_SIZE * COARSE_EPI_MAX_SIZE];
   const int c = blockIdx.x, img = blockIdx.y;
   const int in_plane = size * size;
@@ -129,8 +138,7 @@ extern "C" int tdx_trig_mix(float* out, const float* sample, const float* noise,
                 reinterpret_cast<uintptr_t>(sample)) & 15) == 0, "trig_mix: pointers must be 16-byte aligned");
   int blocks = (int)((numel / 4 + 255) / 256);
   if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-  trig_mix_kernel<<<blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(out, sample, noise, numel, a, b);
-  TDX_CHECK_CUDA(cudaGetLastError());
+  TDX_CHECK_CUDA(launch(trig_mix_kernel, blocks, 256, 0, stream, out, sample, noise, numel, a, b));
   return TDX_OK;
 }
 
@@ -142,9 +150,7 @@ extern "C" int tdx_pack_weighted(float* out, const float* x, const float* w, int
               "pack_weighted: pointers must be 16-byte aligned");
   int bx = (int)((plane / 4 + 255) / 256);
   if (bx > sm_count() * 4) bx = sm_count() * 4;
-  pack_weighted_kernel<<<dim3(bx, n_img), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(out, x, w, channels, plane,
-                                                                                            scale);
-  TDX_CHECK_CUDA(cudaGetLastError());
+  TDX_CHECK_CUDA(launch(pack_weighted_kernel, dim3(bx, n_img), 256, 0, stream, out, x, w, channels, plane, scale));
   return TDX_OK;
 }
 
@@ -154,9 +160,8 @@ extern "C" int tdx_window_to_cond(float* out, const float* packed, int32_t n_img
               w >= 1 && factor >= 1, "window_to_cond: bad arguments");
   int bx = (h * factor * w * factor + 255) / 256;
   if (bx > 1024) bx = 1024;
-  window_to_cond_kernel<<<dim3(bx, keep, n_img), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      out, packed, packed_channels, keep, h, w, factor);
-  TDX_CHECK_CUDA(cudaGetLastError());
+  TDX_CHECK_CUDA(launch(window_to_cond_kernel, dim3(bx, keep, n_img), 256, 0, stream, out, packed, packed_channels, keep,
+                        h, w, factor));
   return TDX_OK;
 }
 
@@ -169,8 +174,7 @@ extern "C" int tdx_coarse_epilogue(float* out, const float* x, const float* mean
               "coarse_epilogue: bad shape (need 1 <= n_img <= 65535, 1 <= size <= 64, pool >= 1 dividing size)");
   TDX_REQUIRE(elev_mode >= POOL_AVG && elev_mode <= POOL_MIN && p5_mode >= POOL_AVG && p5_mode <= POOL_MIN,
               "coarse_epilogue: pool modes must be 0 (avg), 1 (max) or 2 (min)");
-  coarse_epilogue_kernel<<<dim3(COARSE_CH, n_img), COARSE_EPI_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      out, x, means, stds, w, size, pool, elev_mode, p5_mode, sigma_data);
-  TDX_CHECK_CUDA(cudaGetLastError());
+  TDX_CHECK_CUDA(launch(coarse_epilogue_kernel, dim3(COARSE_CH, n_img), COARSE_EPI_THREADS, 0, stream, out, x, means,
+                        stds, w, size, pool, elev_mode, p5_mode, sigma_data));
   return TDX_OK;
 }

@@ -286,11 +286,8 @@ extern "C" int tdx_fbm_perlin(int32_t n_planes, const int32_t* seeds, const floa
     p.lacunarity[k] = lacunarity[k];
     p.gain[k] = gain[k];
   }
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3((unsigned)(((long)h * w + kThreads - 1) / kThreads), (unsigned)n_planes),
-                     dim3(kThreads), 0, reinterpret_cast<cudaStream_t>(stream));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, fbm_kernel, p, (long long)i0, (long long)j0, (int)h, (int)w, out));
+  TDX_CHECK_CUDA(launch(fbm_kernel, dim3((unsigned)(((long)h * w + kThreads - 1) / kThreads), (unsigned)n_planes),
+                        kThreads, 0, stream, p, (long long)i0, (long long)j0, (int)h, (int)w, out));
   return TDX_OK;
 }
 
@@ -342,11 +339,8 @@ extern "C" int tdx_synthetic_map(const double* tables, int32_t n_knots, const in
     imp.has_default = imp_has_default;
   }
   const size_t smem = (raw_input ? 0 : 2 * kFields * (size_t)n_knots * sizeof(double)) + 256 * sizeof(float);
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  fill_launch_config(&cfg, attr, dim3((unsigned)(((long)h * w + kThreads - 1) / kThreads)), dim3(kThreads), smem,
-                     reinterpret_cast<cudaStream_t>(stream));
-  TDX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, synth_kernel, p, imp, tables, raw_input ? 0 : (int)n_knots, (long long)i0,
-                                    (long long)j0, (int)h, (int)w, input, (int)mode, out));
+  TDX_CHECK_CUDA(launch(synth_kernel, (unsigned)(((long)h * w + kThreads - 1) / kThreads), kThreads, smem, stream, p,
+                        imp, tables, raw_input ? 0 : (int)n_knots, (long long)i0, (long long)j0, (int)h, (int)w, input,
+                        (int)mode, out));
   return TDX_OK;
 }
