@@ -16,7 +16,9 @@
 //   warpgroups.  Warpgroup g issues m64nNk16 wgmmas for pixels 64g .. 64g+63 (tile rows 8g .. 8g+7) with the
 //   accumulator in registers, then writes it to a shared-memory staging tile (fp32, [channel][pixel]) from which all
 //   eight warps run the epilogue with one thread per pixel.  The producers keep filling the rings for the next item
-//   while the epilogue runs.
+//   while the epilogue runs.  Cluster-free launches with N <= 128, several items per CTA and no pixel-norm use a
+//   512-thread variant (kOV) instead: w12..w15 are an epilogue warpgroup, handed the staging tile through two
+//   mbarriers, so the MMA warpgroups go straight on to the next item's wgmmas while the epilogue of the last one runs.
 // * Epilogue: each thread owns one pixel; it applies emb-scale+mp_silu / residual mp_sum + clip / pixel-norm and
 //   writes up to three bf16 NC8HW8 outputs (raw, activated, activated+resampled) for the consumers.  Pixel-norm needs
 //   the sum of squares over ALL Cout channels: the Cout/N CTAs of one M tile are then launched as a thread-block
@@ -41,6 +43,7 @@ constexpr int kEpiWarps = 4 * kWQ;                // = the two consumer warpgrou
 constexpr int kChunk = 32;                        // accumulator columns an epilogue warp handles at a time
 constexpr int kGroups = kChunk / 8;               // 8-channel groups (one uint4 of bf16) per chunk
 constexpr int kThreads = 128 + 32 * kEpiWarps;
+constexpr int kOvThreads = kThreads + 128;        // + the epilogue warpgroup of the overlapped variant
 constexpr int kMaxSplit = 8;                      // max CTAs (cluster size) sharing one M tile's pixel-norm statistics
 constexpr int kSmemMisc = 14336;                  // barriers, pixel-norm statistics
 constexpr int kSmemBudget = 227 * 1024;
@@ -259,10 +262,13 @@ struct ConsumerRing {
 
 // One work item's K stages [s0, s1) on the tensor cores.  Consumer warpgroup wg computes pixels 64 wg .. 64 wg + 63
 // against all kN channels of the item, then stores its accumulator into the staging tile stg[channel * kStgLd + pixel].
-template <int kN>
+// kOV: the staging tile is handed to the epilogue warpgroup through two mbarriers -- wait for `stg_empty` (the epilogue
+// has loaded item it - 1 from it), store, arrive on `stg_full` -- instead of a named barrier shared with the epilogue.
+template <int kN, bool kOV>
 __device__ __forceinline__ void mma_item(const IgemmParams& p, const uint8_t* a_ring, const uint8_t* b_ring,
                                          uint64_t* a_full, uint64_t* a_empty, uint64_t* b_full, uint64_t* b_empty,
-                                         ConsumerRing& r, int s0, int s1, bool steady, float* stg) {
+                                         ConsumerRing& r, int s0, int s1, bool steady, float* stg,
+                                         uint64_t* stg_full, uint64_t* stg_empty, int it) {
   const int lane = threadIdx.x & 31, wl = (threadIdx.x >> 5) & 3, wg = (int)(threadIdx.x >> 7) - 1;
   float acc[kN / 2];
 #pragma unroll
@@ -327,7 +333,10 @@ __device__ __forceinline__ void mma_item(const IgemmParams& p, const uint8_t* a_
   }
   wgmma_wait<0>();
   release(pend_a, pend_b);
-  named_bar_sync(13, 32 * kEpiWarps);   // the previous item's epilogue has read the staging tile
+  if constexpr (kOV)
+    mbar_wait(stg_empty, (uint32_t)(it & 1) ^ 1u);
+  else
+    named_bar_sync(13, 32 * kEpiWarps);   // the previous item's epilogue has read the staging tile
   float* dst = stg + 64 * wg + 16 * wl + (lane >> 2);
 #pragma unroll
   for (int j = 0; j < kN / 8; ++j)
@@ -335,16 +344,24 @@ __device__ __forceinline__ void mma_item(const IgemmParams& p, const uint8_t* a_
     for (int i = 0; i < 2; ++i)
 #pragma unroll
       for (int c = 0; c < 2; ++c) dst[(8 * j + 2 * (lane & 3) + c) * kStgLd + 8 * i] = acc[4 * j + 2 * i + c];
-  named_bar_sync(13, 32 * kEpiWarps);
+  if constexpr (kOV) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(stg_full);
+  } else {
+    named_bar_sync(13, 32 * kEpiWarps);
+  }
 }
 
 // kCL = the launch uses clusters (split-K and / or pixel-norm statistics across CTAs).  The many-item launches do not:
 // their instantiation carries none of that code (a shorter epilogue loop, fewer instruction-cache misses).
 // kN = output channels per work item (the wgmma N).
-template <bool kCL, int kN>
-__global__ void __launch_bounds__(kThreads, 1)
+// kOV = overlapped epilogue (cluster-free launches, kN <= 128): warps 12..15 are a third warpgroup that runs the
+// epilogue while the two MMA warpgroups go on to the next item (kOvThreads threads; kEpiWarps then counts MMA warps).
+template <bool kCL, int kN, bool kOV = false>
+__global__ void __launch_bounds__(kOV ? kOvThreads : kThreads, 1)
 igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
              const __grid_constant__ CUtensorMap tm2, const __grid_constant__ IgemmParams p) {
+  static_assert(!kOV || (!kCL && kN <= 128), "the overlapped epilogue is for cluster-free launches with N <= 128");
   extern __shared__ __align__(1024) uint8_t smem[];
   const int ksplit_ = kCL ? p.ksplit : 1;
   const bool cstats_ = kCL && p.cluster_stats;
@@ -356,6 +373,8 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
   uint64_t* b_full = a_empty + kSA;
   uint64_t* b_empty = b_full + kMaxSB;
   uint64_t* x_full = b_empty + kMaxSB;                                // [2] cluster statistics barriers
+  uint64_t* stg_full = x_full + 2;                                    // kOV: staging tile written by the MMA warps
+  uint64_t* stg_empty = stg_full + 1;                                 // kOV: staging tile read by the epilogue
   float* ssq = reinterpret_cast<float*>(bars) + 256;                  // [4 epilogue warps of a pixel][128 pixels]
   float* rss = ssq + 512;                                             // same, for the residual's pixel-norm
   float* stot = rss + 512;                                            // [128] per-pixel totals over the cluster
@@ -382,9 +401,11 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
   }
   if (warp == 2) {
     // all 44 barriers at once, two per lane (one thread initialising them in turn costs ~800 cycles of every launch):
-    // [a_full 3][a_empty 3][b_full 18][b_empty 18][x_full 2], contiguous from `bars`.  Every consumer warp frees a slot.
-    constexpr int kBars = 2 * kSA + 2 * kMaxSB + 2;
+    // [a_full 3][a_empty 3][b_full 18][b_empty 18][x_full 2], contiguous from `bars`, and with kOV [stg_full][stg_empty].
+    // Every MMA warp frees a slot and fills the staging tile; every epilogue warp of kOV empties it.
+    constexpr int kBars = 2 * kSA + 2 * kMaxSB + 2 + (kOV ? 2 : 0);
     static_assert(kBars <= 64, "two barriers per lane");
+    static_assert(kBars * 8 <= 256 * 4, "the barriers sit below the statistics arrays in kSmemMisc");
     const int x_full0 = 2 * kSA + 2 * kMaxSB;
 #pragma unroll
     for (int k = 0; k < 2; ++k) {
@@ -393,6 +414,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
         uint32_t count = 1;
         if ((i >= kSA && i < 2 * kSA) || (i >= 2 * kSA + kMaxSB && i < x_full0)) count = kEpiWarps;
         if (i >= x_full0) count = p.xsplit > 1 ? (uint32_t)(p.xsplit - 1) * 128u : 1u;
+        if (kOV && i >= x_full0 + 2) count = i == x_full0 + 2 ? kEpiWarps : 4u;
         mbar_init(&bars[i], count);
       }
     }
@@ -494,19 +516,37 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
     if (ksplit_ > 1) cluster_sync_all();
   } else if (warp < 4) {
     if (ksplit_ > 1) cluster_sync_all();
+  } else if (kOV && warp < 12) {
+    // ------------------------------------------------------------------ kOV: MMA warpgroups only
+    TileWalk tw;
+    tw.init(p);
+    ConsumerRing ring = {0, 0, 0u, 0u};
+    int s0, s1;
+    stage_range(p, tw.kpart, s0, s1);
+    int it = 0;
+    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x, ++it) {
+      if (warp == 4 && lane == 0) TDX_TRACE(1, it);
+      mma_item<kN, kOV>(p, a_ring, b_ring, a_full, a_empty, b_full, b_empty, ring, s0, s1, p.resident && it > 0, stg,
+                        stg_full, stg_empty, it);
+      if (warp == 4 && lane == 0) TDX_TRACE(2, it);
+    }
   } else {
     // ------------------------------------------------------------------ consumers: MMA, then the epilogue
     // In the epilogue warp w handles quadrant q = w & 3 of the staging tile (pixels q*32 .. q*32+31, one per lane); the
-    // kWQ warps of a quadrant (wq = 0 .. kWQ-1) take the item's kChunk-column chunks round-robin.
+    // kWQ warps of a quadrant (wq = 0 .. kWQ-1) take the item's kChunk-column chunks round-robin.  With kOV the one
+    // epilogue warp of a quadrant takes every chunk (wq = 0, step 1); the residual's pixel-norm keeps the kWQ partial
+    // sums apart, so that they are added in the same order as with kWQ warps.
     pdl_wait();  // residual / cvec come from earlier kernels; our stores must not race their readers
     const int q = warp & 3;
-    const int wq = (warp - 4) >> 2;
+    const int wq = kOV ? 0 : (warp - 4) >> 2;
+    constexpr int kStep = kOV ? 1 : kWQ;   // chunk stride of one epilogue warp
     const int m = q * 32 + lane;
     const int y = m >> 3, x = m & 7;
     const int C8 = p.cout >> 3;
-    const bool need_norm = (p.epi & TDX_EPI_PNORM) || p.out[0].kind == TDX_OUT_PNORM_SILU ||
+    // (kOV launches have no pixel-norm statistics: the host sends those to the kernel with eight epilogue warps)
+    const bool need_norm = !kOV && ((p.epi & TDX_EPI_PNORM) || p.out[0].kind == TDX_OUT_PNORM_SILU ||
                            p.out[1].kind == TDX_OUT_PNORM_SILU || p.out[2].kind == TDX_OUT_PNORM_SILU ||
-                           p.rms_out != nullptr;
+                           p.rms_out != nullptr);
     const uint32_t my_rank = cstats_ ? cluster_ctarank() : 0;
     TileWalk tw;
     tw.init(p);
@@ -573,8 +613,10 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
     // The values an item needs from global memory before it can touch its accumulator are requested ONE ITEM AHEAD
     // (`fetch_ahead`, called where the current item has consumed them): the residual's first-chunk channels or the
     // modulation vector's first chunk (`pre`) and the residual's pixel-norm factor (`rinv_pre`), so that their first use
-    // does not wait on a global load.
-    constexpr int kPreN = (kChunk / 4 > kGroups) ? kChunk / 4 : kGroups;
+    // does not wait on a global load.  The epilogue warps of kOV have 128 registers, not 168: they fetch the first two
+    // uint4 of that chunk ahead, not all of it.
+    constexpr int kPreN = kOV ? 2 : ((kChunk / 4 > kGroups) ? kChunk / 4 : kGroups);
+    constexpr int kPreG = kPreN < kGroups ? kPreN : kGroups;   // residual groups among them
     uint4 pre[kPreN];
     const uint4* rbase_pre = nullptr;
     float rinv_pre = 1.f;
@@ -585,7 +627,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
       if (cv_ahead) {
         const uint4* cp = reinterpret_cast<const uint4*>(p.cvec + (size_t)t.img * p.cout + chbase + wq * kChunk);
 #pragma unroll
-        for (int j = 0; j < kChunk / 4; ++j) pre[j] = (wq < nchunks) ? __ldg(cp + j) : make_uint4(0, 0, 0, 0);
+        for (int j = 0; j < kPreN; ++j) pre[j] = (wq < nchunks) ? __ldg(cp + j) : make_uint4(0, 0, 0, 0);
         return;
       }
       if (!has_resid) return;
@@ -596,7 +638,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
       if (p.resid_inv) rinv_pre = vld ? __ldg(p.resid_inv + item_off(rinv_spec, t)) : 0.f;
       const uint4* rptr = rbase_pre + (size_t)((chbase >> 3) + wq * kGroups) * rplane;
 #pragma unroll
-      for (int g = 0; g < kGroups; ++g)
+      for (int g = 0; g < kPreG; ++g)
         pre[g] = (vld && wq < nchunks) ? __ldg(rptr + (size_t)g * rplane) : make_uint4(0, 0, 0, 0);
     };
     if (ahead) fetch_ahead(tw);
@@ -605,9 +647,14 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
       const int img = tw.img;
       const int Y = tw.ty * kTileH + y, X = tw.tx * kTileW + x;
       const bool valid = (Y < p.H) && (X < p.W);
-      if (warp == 4 && lane == 0) TDX_TRACE(1, it);
-      mma_item<kN>(p, a_ring, b_ring, a_full, a_empty, b_full, b_empty, ring, s0, s1, p.resident && it > 0, stg);
-      if (warp == 4 && lane == 0) TDX_TRACE(2, it);
+      if constexpr (kOV) {
+        mbar_wait(stg_full, (uint32_t)(it & 1));
+      } else {
+        if (warp == 4 && lane == 0) TDX_TRACE(1, it);
+        mma_item<kN, kOV>(p, a_ring, b_ring, a_full, a_empty, b_full, b_empty, ring, s0, s1, p.resident && it > 0, stg,
+                          stg_full, stg_empty, it);
+        if (warp == 4 && lane == 0) TDX_TRACE(2, it);
+      }
 
       // ---------------- split-K: the ksplit CTAs of a cluster each hold a partial sum of the same 128 x ncta tile.
       // Reduce-scatter through an L2-resident fp32 workspace: every part publishes the column slices the other parts
@@ -661,18 +708,37 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
             unpack_bf16x2(u.z, a, b); ss = fmaf(a, a, fmaf(b, b, ss));
             unpack_bf16x2(u.w, a, b); ss = fmaf(a, a, fmaf(b, b, ss));
           };
-          if (valid) {
-            for (int g0 = wq * 2; g0 < C8; g0 += 2 * kWQ) {
-              const uint4 u0 = __ldg(rbase + (size_t)g0 * rplane), u1 = __ldg(rbase + (size_t)(g0 + 1) * rplane);
-              sq8(u0);
-              sq8(u1);
-            }
-          }
-          rss[wq * 128 + m] = ss;
-          named_bar_sync(9 + q, 32 * kWQ);
-          ss = 0.f;
+          if constexpr (kOV) {
+            float part[kWQ];
 #pragma unroll
-          for (int w = 0; w < kWQ; ++w) ss += rss[w * 128 + m];
+            for (int w = 0; w < kWQ; ++w) {
+              ss = 0.f;
+              if (valid) {
+                for (int g0 = w * 2; g0 < C8; g0 += 2 * kWQ) {
+                  const uint4 u0 = __ldg(rbase + (size_t)g0 * rplane), u1 = __ldg(rbase + (size_t)(g0 + 1) * rplane);
+                  sq8(u0);
+                  sq8(u1);
+                }
+              }
+              part[w] = ss;
+            }
+            ss = 0.f;
+#pragma unroll
+            for (int w = 0; w < kWQ; ++w) ss += part[w];
+          } else {
+            if (valid) {
+              for (int g0 = wq * 2; g0 < C8; g0 += 2 * kWQ) {
+                const uint4 u0 = __ldg(rbase + (size_t)g0 * rplane), u1 = __ldg(rbase + (size_t)(g0 + 1) * rplane);
+                sq8(u0);
+                sq8(u1);
+              }
+            }
+            rss[wq * 128 + m] = ss;
+            named_bar_sync(9 + q, 32 * kWQ);
+            ss = 0.f;
+#pragma unroll
+            for (int w = 0; w < kWQ; ++w) ss += rss[w * 128 + m];
+          }
           rscale = p.resid_scale * inv_rms(ss, p.inv_cout);
         }
         // this thread's pixel in each output (inactive: out of the image, or an odd pixel of a 2x-downsampled output)
@@ -693,7 +759,8 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
           if (p.epi & TDX_EPI_EMB_SILU) {
 #pragma unroll
             for (int i = 0; i < kChunk; i += 4) {
-              const uint4 cu = (cv_ahead && ck == wq) ? pre[i >> 2] : __ldg(reinterpret_cast<const uint4*>(cvb + ck * kChunk + i));
+              const uint4 cu = (cv_ahead && ck == wq && (i >> 2) < kPreN) ? pre[i >> 2]
+                                                                          : __ldg(reinterpret_cast<const uint4*>(cvb + ck * kChunk + i));
               const float4 c4 = make_float4(__uint_as_float(cu.x), __uint_as_float(cu.y), __uint_as_float(cu.z), __uint_as_float(cu.w));
               v[i + 0] = mp_silu_f(v[i + 0] * c4.x);
               v[i + 1] = mp_silu_f(v[i + 1] * c4.y);
@@ -705,7 +772,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
             const uint4* rptr = rbase + (size_t)((chbase >> 3) + ck * kGroups) * rplane;
 #pragma unroll
             for (int g = 0; g < kGroups; ++g) {
-              uint4 u = (ck == wq) ? pre[g] : (valid ? __ldg(rptr + (size_t)g * rplane) : make_uint4(0, 0, 0, 0));
+              uint4 u = (ck == wq && g < kPreG) ? pre[g] : (valid ? __ldg(rptr + (size_t)g * rplane) : make_uint4(0, 0, 0, 0));
               float rr[8];
               unpack_bf16x2(u.x, rr[0], rr[1]);
               unpack_bf16x2(u.y, rr[2], rr[3]);
@@ -780,11 +847,15 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
 #pragma unroll 1
         for (int pass = need_norm ? 0 : 1; pass < 2; ++pass) {
 #pragma unroll 1
-          for (int ck = wq; ck < nchunks; ck += kWQ) {
+          for (int ck = wq; ck < nchunks; ck += kStep) {
             if (pass == 0 || !reuse) {
               compute_v(ck, v);
               // `pre` (chunk wq of this item) has just been used for the last time: request the next item's
               if (ck == wq && (reuse || pass == 1) && more) fetch_ahead(tn);
+              if (kOV && ck == nchunks - 1) {
+                __syncwarp();   // the item's last read of the staging tile: the MMA warps may overwrite it
+                if (lane == 0) mbar_arrive(stg_empty);
+              }
             }
             if (pass == 0) {
 #pragma unroll
@@ -800,7 +871,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
           }
         }
       }
-      if (warp == 4 && lane == 0) TDX_TRACE(4, it);
+      if (warp == (kOV ? 12 : 4) && lane == 0) TDX_TRACE(4, it);
     }
   }
 
@@ -825,10 +896,23 @@ static int ensure_scratch(float** ws);
 
 typedef decltype(&igemm_kernel<false, 64>) IgemmKernel;
 
-static IgemmKernel igemm_kernel_for(bool cluster, int n) {
+// Debug: run the cluster-free N <= 128 launches on the serial-epilogue kernel (tests compare the two bit for bit).
+static bool g_serial_epilogue = false;
+
+// Launches that overlap the epilogue with the next item's MMAs: cluster-free with N <= 128, whose accumulator (32 or 64
+// registers per thread) leaves room for a third warpgroup under the 128-register cap of 512 threads; more than one
+// item per CTA (with one there is nothing to overlap, and eight epilogue warps finish it sooner than four); no
+// pixel-norm statistics (measured: their two passes over the staging tile on four warps take longer than the MMAs they
+// would hide).
+static bool overlapped(bool cluster, int n, bool multi_round, bool norm) {
+  return !cluster && n <= 128 && multi_round && !norm;
+}
+
+static IgemmKernel igemm_kernel_for(bool cluster, int n, bool ov) {
   switch (n) {
-    case 64: return cluster ? igemm_kernel<true, 64> : igemm_kernel<false, 64>;
-    case 128: return cluster ? igemm_kernel<true, 128> : igemm_kernel<false, 128>;
+    case 64: return cluster ? igemm_kernel<true, 64> : (ov ? igemm_kernel<false, 64, true> : igemm_kernel<false, 64>);
+    case 128:
+      return cluster ? igemm_kernel<true, 128> : (ov ? igemm_kernel<false, 128, true> : igemm_kernel<false, 128>);
     case 192: return cluster ? igemm_kernel<true, 192> : igemm_kernel<false, 192>;
     default: return cluster ? igemm_kernel<true, 256> : igemm_kernel<false, 256>;
   }
@@ -839,8 +923,9 @@ int igemm_prepare() {
   if (first_use_on_device(seen)) {
     for (int n = 64; n <= 256; n += 64)
       for (int cl = 0; cl < 2; ++cl)
-        TDX_CHECK_CUDA(
-            cudaFuncSetAttribute(igemm_kernel_for(cl, n), cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
+        for (int ov = 0; ov < (overlapped(cl, n, true, false) ? 2 : 1); ++ov)
+          TDX_CHECK_CUDA(cudaFuncSetAttribute(igemm_kernel_for(cl, n, ov), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              kSmemBudget));
   }
   float* ws;
   return ensure_scratch(&ws);
@@ -952,7 +1037,10 @@ static ItemShape choose_item_shape(int cout, int tiles, int stages, int chunks, 
       double t = mma;
       if (l2 > t) t = l2;
       if (per_sm > t) t = per_sm;
-      t += epi + red;
+      if (overlapped(csize > 1, n, rounds > 1, norm))
+        t = (epi > t ? epi : t) + red;   // the epilogue runs beside the next item's MMAs
+      else
+        t += epi + red;
       if (t < best) { best = t; bs = {n, resident, sa, sb, ks}; }
     }
   }
@@ -1035,7 +1123,8 @@ int igemm_launch(const TdxIgemmDesc& d, const CUtensorMap* tms, cudaStream_t str
   const CUtensorMap& t0 = tms[0];
   const CUtensorMap& t1 = tms[d.n_seg > 1 ? 1 : 0];
   const CUtensorMap& t2 = tms[d.n_seg > 2 ? 2 : 0];
-  TDX_CHECK_CUDA(launch_clustered(cluster, igemm_kernel_for(cluster > 1, p.ncta), grid, kThreads,
+  const bool ov = overlapped(cluster > 1, p.ncta, p.num_items > grid, norm) && !g_serial_epilogue;
+  TDX_CHECK_CUDA(launch_clustered(cluster, igemm_kernel_for(cluster > 1, p.ncta, ov), grid, ov ? kOvThreads : kThreads,
                                   smem < 120 * 1024 ? 120 * 1024 : smem, stream, t0, t1, t2, p));
   return TDX_OK;
 }
@@ -1094,6 +1183,10 @@ extern "C" void tdx_debug_set_igemm_timeline(void* device_u64_pairs, int capacit
   tdx::g_timeline_idx = 0;
   tdx::g_timeline_cap = capacity;
 }
+
+// Debug (tests/test_igemm_overlap_gpu.py): nonzero = launches made from now on run their epilogue after the MMAs on the
+// same warps even where the overlapped kernel applies; the launch plan stays the same.
+extern "C" void tdx_debug_igemm_serial_epilogue(int32_t on) { tdx::g_serial_epilogue = on != 0; }
 
 extern "C" int tdx_igemm_choose_n(int32_t c_out, int32_t n_img, int32_t height, int32_t width,
                                   const int32_t* a_channels, const int32_t* a_taps, int32_t n_seg) {
