@@ -78,7 +78,9 @@ def device_sm_count() -> int:
 def plan_of(case: Case, sm_count: int | None = None) -> dict:
     """The launch plan igemm_launch makes for this case on the current device: work-item width N, split-K factor,
     resident weights or ring depth SB, cluster size, and the grid it derives from them (rounds = work items per CTA,
-    `partial` = the last round leaves some CTAs idle).  `ragged` = the height is not a multiple of the 16-row tile."""
+    `partial` = the last round leaves some CTAs idle).  `ragged` = the height is not a multiple of the 16-row tile.
+    `ov` = igemm_launch runs it on the overlapped-epilogue kernel (its `overlapped()`: cluster-free, N <= 128, more
+    than one round, no pixel-norm statistics), otherwise on the serial-epilogue kernel."""
     ch = (C.c_int32 * 3)(*[c for c, _ in case.segs], *([0] * (3 - len(case.segs))))
     tp = (C.c_int32 * 3)(*[t for _, t in case.segs], *([0] * (3 - len(case.segs))))
     n_item = case.n_item or L.igemm_choose_n(case.cout, case.n, case.h, case.w, case.segs)
@@ -95,7 +97,8 @@ def plan_of(case: Case, sm_count: int | None = None) -> dict:
     grid -= grid % (nsplit * ks)
     rounds = -(-items // grid)
     return dict(N=N, ks=ks, resident=resident, SB=sb, cluster=cluster, nsplit=nsplit, items=items, grid=grid,
-                rounds=rounds, partial=items % grid != 0, ragged=case.h % TILE_H != 0)
+                rounds=rounds, partial=items % grid != 0, ragged=case.h % TILE_H != 0,
+                ov=cluster == 1 and N <= 128 and rounds > 1 and not norm)
 
 
 def plan_class(p: dict) -> tuple:
@@ -108,6 +111,17 @@ def plan_label(cls: tuple) -> str:
     N, ks, res, sb, cl, multi, ragged = cls
     return (f"N{N}-ks{ks}-{'res' if res else 'SB'}{sb}-cl{cl}-{'multi' if multi else 'one'}"
             f"{'-ragged' if ragged else ''}")
+
+
+def plan_variant(p: dict) -> tuple:
+    """plan_class + (partial last round, overlapped-epilogue kernel): on the overlapped kernel the last round, partial
+    or not, is where the MMA warpgroups and the epilogue warpgroup fall out of step."""
+    return plan_class(p) + (p["partial"], p["ov"])
+
+
+def variant_label(v: tuple) -> str:
+    *cls, partial, ov = v
+    return f"{plan_label(tuple(cls))}{'-partial' if partial else ''}-{'ov' if ov else 'serial'}"
 
 
 def make_inputs(case: Case, device):

@@ -25,7 +25,7 @@ from terrain_diffusion_b200.models import EDMAutoencoder
 from terrain_diffusion_b200.models.plan import FoldedWeights, autoencoder_decoder_plan
 from tests._igemm_ref import case_from_desc, check_case, plan_class, plan_label, plan_of, report
 from tests.test_autoencoder_cpu import _record
-from tests.test_igemm_plans_gpu import representatives
+from tests._igemm_surface import representatives
 
 pytestmark = pytest.mark.gpu
 G = np.load(Path(__file__).resolve().parent / "golden" / "autoencoder_golden.npz")

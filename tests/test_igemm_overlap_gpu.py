@@ -4,21 +4,24 @@ serial-epilogue kernel, bit for bit.
 
 Both kernels issue the same MMAs in the same order and the same epilogue arithmetic in the same order, so every output
 byte must agree.  The serial kernel is selected through the debug hook tdx_debug_igemm_serial_epilogue; the launch plan
-is the same either way.  Cases: every (plan class, epilogue signature) of the decoder's 256^2 and 128^2 launches in a
-one-tile and a 16-tile forward (the bench's shapes), plus hand-written cases for the epilogue paths and item counts
-those forwards may not reach on a given GPU.
+is the same either way.  Cases: every (plan class, epilogue signature) of the decoder's overlapped 256^2 and 128^2
+launches in a one-tile and a 16-tile forward (the bench's shapes); then every other (plan variant, epilogue signature)
+group of the shape surface (tests/_igemm_surface.py) that runs on the overlapped kernel; plus hand-written cases for the
+epilogue paths and item counts the surface may not reach on a given GPU.
 """
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 import functools
 
 import pytest
 import torch
 
 from terrain_diffusion_b200 import _lib as L
-from tests._capture import capture_forward, layer_of
-from tests._igemm_ref import Case, case_from_desc, make_inputs, needs_norm, plan_class, plan_label, plan_of, run_cuda
+from tests._igemm_ref import Case, make_inputs, plan_class, plan_label, plan_of, report, run_cuda
+from tests._igemm_surface import (BENCH_TILE, BENCH_TILES, Forward, epilogue_signature, gpu_tests_selected,
+                                  group_key, group_representatives, launches, new_groups)
 
 pytestmark = pytest.mark.gpu
 
@@ -51,44 +54,41 @@ HAND_CASES = [
 ]
 
 
-def overlapped(case: Case, plan: dict) -> bool:
-    """Whether igemm_launch runs this launch on the overlapped kernel."""
-    return plan["cluster"] == 1 and plan["N"] <= 128 and plan["rounds"] > 1 and not needs_norm(case)
-
-
-def epilogue_signature(c: Case) -> tuple:
-    return (c.epi, c.resid_spatial if c.epi & R else None, c.resid_pnorm, c.resid_inv, c.rms_out,
-            tuple((k, s) for k, s, _ in c.outs), c.clip > 0, tuple(t for _, t in c.segs))
-
-
 @functools.lru_cache(maxsize=None)
 def decoder_cases() -> tuple:
     """The fewest-MAC launch of every (plan class, epilogue signature) among the decoder's overlapped 256^2 and 128^2
-    launches at batch 1 and 16."""
+    launches at the bench's 1 and 16 tiles."""
     groups: dict = {}
-    for n in (1, 16):
-        prog = capture_forward("decoder", n, 256)
-        for d in prog.igemm():
-            if d.height not in (256, 128):
-                continue
-            c = case_from_desc(d, name=f"decoder_b{n}:{layer_of(prog, d)}")
-            p = plan_of(c)
-            if not overlapped(c, p):
-                continue
-            key = (plan_class(p), epilogue_signature(c))
-            if key not in groups or c.macs < groups[key].macs:
-                groups[key] = c
-    cases = []
-    for (cls, _), c in sorted(groups.items(), key=lambda kv: str(kv[0])):
-        c.name = f"{plan_label(cls)}-{c.name}"
-        cases.append(c)
-    return tuple(cases)
+    for la in launches():
+        if la.forward.model != "decoder" or la.forward.hw != BENCH_TILE or la.forward.n not in BENCH_TILES:
+            continue
+        if la.case.h not in (256, 128) or not la.plan["ov"]:
+            continue
+        key = (plan_class(la.plan), epilogue_signature(la.case))
+        if key not in groups or la.case.macs < groups[key].macs:
+            groups[key] = dataclasses.replace(la.case, name=f"decoder_b{la.forward.n}:{la.layer}")
+    return tuple(dataclasses.replace(c, name=f"{plan_label(cls)}-{c.name}")
+                 for (cls, _), c in sorted(groups.items(), key=lambda kv: str(kv[0])))
+
+
+@functools.lru_cache(maxsize=None)
+def surface_cases() -> tuple:
+    """The representative of every surface group on the overlapped kernel that decoder_cases() leaves out."""
+    done = {group_key(c, plan_of(c)) for c in decoder_cases()}
+    return tuple(c for c in group_representatives() if plan_of(c)["ov"] and group_key(c, plan_of(c)) not in done)
 
 
 def pytest_generate_tests(metafunc):
-    if metafunc.function.__name__ == "test_decoder_plan_overlapped_matches_serial":
-        cases = decoder_cases() if torch.cuda.is_available() else ()
-        metafunc.parametrize("case", cases, ids=lambda c: c.name)
+    cases = {"test_decoder_plan_overlapped_matches_serial": decoder_cases,
+             "test_surface_plan_overlapped_matches_serial": surface_cases}.get(metafunc.function.__name__)
+    if cases is not None:
+        metafunc.parametrize("case", cases() if gpu_tests_selected(metafunc.config) else (), ids=lambda c: c.name)
+
+
+@pytest.fixture(scope="module")
+def compared() -> set:
+    """Names of the cases found bit-identical to the serial kernel in this session."""
+    return set()
 
 
 def _serial(on: bool) -> None:
@@ -103,7 +103,7 @@ def _bits(t: torch.Tensor) -> torch.Tensor:
 
 
 def check_bit_identical(case: Case) -> None:
-    assert overlapped(case, plan_of(case)), f"{case.name}: plan {plan_of(case)} does not run the overlapped kernel"
+    assert plan_of(case)["ov"], f"{case.name}: plan {plan_of(case)} does not run the overlapped kernel"
     inputs = make_inputs(case, "cuda:0")
     try:
         _serial(True)
@@ -119,8 +119,14 @@ def check_bit_identical(case: Case) -> None:
         assert diff == 0, f"{case.name} {what}: {diff} elements differ from the serial-epilogue kernel"
 
 
-def test_decoder_plan_overlapped_matches_serial(case):
+def test_decoder_plan_overlapped_matches_serial(case, compared):
     check_bit_identical(case)
+    compared.add(case.name)
+
+
+def test_surface_plan_overlapped_matches_serial(case, compared):
+    check_bit_identical(case)
+    compared.add(case.name)
 
 
 @pytest.mark.parametrize("case", HAND_CASES, ids=lambda c: c.name)
@@ -128,11 +134,24 @@ def test_hand_case_overlapped_matches_serial(case):
     check_bit_identical(case)
 
 
-def test_cases_cover_the_epilogue_paths():
-    """Between them the cases reach several rounds per CTA with a partial last round, both N, and every epilogue
-    feature the overlapped kernel takes."""
-    cases = list(decoder_cases()) + HAND_CASES
+def test_cases_cover_the_epilogue_paths(request, compared):
+    """Every surface group on the overlapped kernel is compared with the serial kernel by one of the two parametrized
+    tests above (or here, if they have not compared it in this session), and between them the cases reach several
+    rounds per CTA with a partial last round, both N, and every epilogue feature the overlapped kernel takes.  Writes
+    the number of overlapped groups, and of those no PRODUCT forward reaches, to the terminal (also under -q)."""
     assert decoder_cases(), "no overlapped 256^2 / 128^2 launch in the decoder forward"
+    ov = list(decoder_cases()) + list(surface_cases())
+    keys = {group_key(la.case, la.plan) for la in launches() if la.plan["ov"]}
+    compared_keys = {group_key(c, plan_of(c)) for c in ov}
+    assert keys <= compared_keys, sorted(map(str, keys - compared_keys))
+    for c in ov:
+        if c.name not in compared:
+            check_bit_identical(c)
+    new = new_groups()
+    report(request.config, [f"igemm overlapped kernel: {len(keys)} surface groups ({len(ov)} cases) bit-identical to "
+                            f"the serial kernel, {sum(1 for k in keys if k in new)} of them reached by no PRODUCT "
+                            f"forward; {len(HAND_CASES)} hand-written cases"])
+    cases = ov + HAND_CASES
     plans = [plan_of(c) for c in cases]
     features = {
         "several rounds, partial last": any(p["rounds"] >= 3 and p["partial"] for p in plans),

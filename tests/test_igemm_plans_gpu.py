@@ -1,44 +1,28 @@
-"""Every implicit-GEMM launch plan the shipped models run, replayed against the fp64 reference (tests/_igemm_ref.py).
+"""Every implicit-GEMM launch plan the package runs, replayed against the fp64 reference (tests/_igemm_ref.py).
 
-The launch descriptors of the product's forwards (PRODUCT) are recorded on the host (tests/_capture.py), planned with
-this GPU's SM count and cluster occupancy, and grouped by (plan class, epilogue signature).  The smallest launch of
-each group runs through tdx_igemm_run with fresh bf16-exact inputs, guarded outputs and the per-element bound, so an
-error in one layer, tile row or cluster rank fails here at that layer instead of being diluted in a whole-model
-comparison.  HAND_CASES add the paths the product may not reach on a given GPU.
+The launch descriptors of every forward on the shape surface (tests/_igemm_surface.py: the WorldPipeline stages at
+their padded batches, bench.py, the evaluation batches and the tiled samplers at every `tile_batch`) are recorded on the
+host, planned with this GPU's SM count and cluster occupancy, and grouped by launch plan and epilogue signature.  The
+smallest launch of each group runs through tdx_igemm_run with fresh bf16-exact inputs, guarded outputs and the
+per-element bound, so an error in one layer, tile row, cluster rank or last partial round fails here at that layer
+instead of being diluted in a whole-model comparison.  The PRODUCT forwards' (plan class, epilogue signature) groups
+run first; every finer (plan variant, epilogue signature) group of the surface that they leave out runs after them.
+HAND_CASES add the paths the surface may not reach on a given GPU.
 """
 from __future__ import annotations
 
 import collections
-import functools
+import textwrap
 
 import pytest
 import torch
 
 from terrain_diffusion_b200 import _lib as L
-from tests._capture import capture_forward, layer_of
-from tests._igemm_ref import (Case, case_from_desc, check_case, needs_norm, plan_class, plan_label, plan_of,
-                              report)
+from tests._igemm_ref import Case, check_case, needs_norm, plan_of, plan_variant, report, variant_label
+from tests._igemm_surface import (gpu_tests_selected, group_key, launches, new_groups, product_representatives,
+                                  surface, surface_representatives)
 
 pytestmark = pytest.mark.gpu
-
-PRODUCT = [
-    # (source, model, batch, tile size)
-    ("bench_tiles1", "decoder", 1, 256),           # bench.py (decoder solve, 256^2 tiles)
-    ("bench_tiles16", "decoder", 16, 256),
-    ("world_decoder_b1", "decoder", 1, 512),       # WorldPipeline decoder windows of 512, batches 1-16
-    ("world_decoder_b8", "decoder", 8, 512),
-    ("world_decoder_b16", "decoder", 16, 512),
-    ("decoder_64", "decoder", 1, 64),
-    ("decoder_128_b2", "decoder", 2, 128),
-    ("latent_b1", "base", 1, 64),                  # latent stage, batches 1-16 of 64^2 tiles
-    ("latent_b2", "base", 2, 64),
-    ("latent_b16", "base", 16, 64),
-    ("guided_main_b40", "base", 40, 64),           # guided base diffusion: 40 tiles, main model and guide
-    ("guide_b16", "guide", 16, 64),
-    ("guided_guide_b40", "guide", 40, 64),
-    ("coarse_b1", "coarse", 1, 64),
-    ("coarse_b16", "coarse", 16, 64),
-]
 
 E, R, P = L.EPI_EMB_SILU, L.EPI_RESID, L.EPI_PNORM
 RAW, SILU, PSILU = L.OUT_RAW, L.OUT_SILU, L.OUT_PNORM_SILU
@@ -63,76 +47,11 @@ HAND_CASES = [
 ]
 
 
-def epilogue_signature(c: Case) -> tuple:
-    """Epilogue flags, residual mode, pixel-norm side planes, outputs (kind, spatial), clip on/off, tap pattern."""
-    has_resid = bool(c.epi & R)
-    return (c.epi, c.resid_spatial if has_resid else None, c.resid_pnorm if has_resid else None, c.resid_inv,
-            c.rms_out, tuple((k, s) for k, s, _ in c.outs), c.clip > 0, tuple(t for _, t in c.segs))
-
-
-def _signature_label(sig) -> str:
-    epi, rsp, rpn, rinv, rms, outs, clip, taps = sig
-    parts = ["e" + str(epi)]
-    if rsp is not None:
-        parts.append(f"r{rsp}{'inv' if rinv else ('pn' if rpn else '')}")
-    if rms:
-        parts.append("rms")
-    parts.append("o" + "".join(f"{k}{s}" for k, s in outs))
-    if clip:
-        parts.append("clip")
-    parts.append("t" + "".join(str(t) for t in taps))
-    return ".".join(parts)
-
-
-def product_launches() -> list:
-    """[(source, layer, case, plan)] for every igemm launch of PRODUCT, planned on this device."""
-    out = []
-    for source, model, n, hw in PRODUCT:
-        prog = capture_forward(model, n, hw)
-        for d in prog.igemm():
-            c = case_from_desc(d, name=f"{source}:{layer_of(prog, d)}")
-            out.append((source, layer_of(prog, d), c, plan_of(c)))
-    return out
-
-
-def representatives(launches) -> list:
-    """The smallest launch (fewest MACs) of every (plan class, epilogue signature) group, as a named Case."""
-    groups: dict = {}
-    for source, layer, c, p in launches:
-        key = (plan_class(p), epilogue_signature(c))
-        if key not in groups or c.macs < groups[key][0].macs:
-            groups[key] = (c, p)
-    reps = []
-    for (cls, sig), (c, p) in sorted(groups.items(), key=lambda kv: (kv[0][0], str(kv[0][1]))):
-        c.name = f"{plan_label(cls)}-{_signature_label(sig)}-{c.name}"
-        reps.append(c)
-    return reps
-
-
-@functools.lru_cache(maxsize=None)
-def product() -> tuple:
-    """(launches, representatives) of PRODUCT on this GPU, recorded once per session."""
-    launches = product_launches()
-    return launches, representatives(launches)
-
-
-def _gpu_tests_selected(config) -> bool:
-    """Whether this run executes gpu-marked tests: only then is the product recorded (it folds four models)."""
-    if not torch.cuda.is_available():
-        return False
-    expr = config.getoption("markexpr")
-    if not expr:
-        return True
-    try:
-        from _pytest.mark.expression import Expression
-        return bool(Expression.compile(expr).evaluate(lambda name, **kw: name == "gpu"))
-    except Exception:
-        return True
-
-
 def pytest_generate_tests(metafunc):
-    if metafunc.function.__name__ == "test_product_plan_matches_fp64_reference":
-        reps = product()[1] if _gpu_tests_selected(metafunc.config) else []
+    cases = {"test_product_plan_matches_fp64_reference": product_representatives,
+             "test_surface_plan_matches_fp64_reference": surface_representatives}.get(metafunc.function.__name__)
+    if cases is not None:
+        reps = cases() if gpu_tests_selected(metafunc.config) else ()
         metafunc.parametrize("case", reps, ids=lambda c: c.name)
 
 
@@ -150,27 +69,54 @@ def test_product_plan_matches_fp64_reference(case, margins):
     check_case(case, torch.device("cuda:0"), margins)
 
 
+def test_surface_plan_matches_fp64_reference(case, margins):
+    check_case(case, torch.device("cuda:0"), margins)
+
+
 @pytest.mark.parametrize("case", HAND_CASES, ids=lambda c: c.name)
 def test_hand_written_plan_matches_fp64_reference(case, margins):
     check_case(case, torch.device("cuda:0"), margins)
 
 
-def test_every_product_plan_class_is_covered(request):
-    """Every plan class the product reaches on this GPU is replayed above, and so is each path listed in HAND_CASES.
-    Writes one line per class to the terminal (also under -q): launches in PRODUCT and the case that covers it."""
-    launches, reps = product()
-    assert launches, "no product launches recorded"
+def test_every_product_plan_class_is_covered(request, margins):
+    """Every (plan variant, epilogue signature) group of the surface is replayed against fp64 by one of the two
+    parametrized tests above (or here, if they have not replayed it in this session), and each path listed in
+    HAND_CASES is reached.  Writes to the terminal (also under -q): forwards, launches and groups; the groups the
+    hand-picked PRODUCT forwards do not reach, per first source reaching them; the groups on the overlapped kernel; the
+    worst per-element error; and one line per plan variant with its launch count and the case that covers it."""
+    runs = launches()
+    reps = list(product_representatives()) + list(surface_representatives())
+    assert runs, "no launches recorded"
+    keys = {group_key(la.case, la.plan) for la in runs}
+    replayed = {group_key(c, plan_of(c)) for c in reps}
+    assert keys <= replayed, sorted(map(str, keys - replayed))
+    for c in reps:
+        if c.name not in margins:
+            check_case(c, torch.device("cuda:0"), margins)
+
+    new = new_groups()
+    first = collections.Counter(sources[0] for sources in new.values())
+    ov = [k for k in keys if k[0][-1]]
+    worst = max((c.name for c in reps), key=margins.get)
+    lines = [f"igemm surface: {len(surface())} forwards, {len(runs)} launches, {len(keys)} (plan variant, epilogue) "
+             f"groups, every one replayed against fp64 by {len(reps)} cases; {len(HAND_CASES)} hand-written cases",
+             f"  {len(new)} groups no PRODUCT forward reaches, by the first source that does (WorldPipeline, bench, "
+             f"evaluation, tiled samplers):"]
+    order = [s for sources in surface().values() for s in sources]
+    lines += textwrap.wrap(" ".join(f"{s}={first[s]}" for s in sorted(first, key=order.index)), 116,
+                           initial_indent="    ", subsequent_indent="    ")
+    lines += [f"  {len(ov)} groups run the overlapped-epilogue kernel, {sum(1 for k in ov if k in new)} of them new",
+              f"  worst per-element error over the groups: {margins[worst]:.3f} of the bound ({worst})"]
+
     run = [(c, plan_of(c)) for c in reps + HAND_CASES]
     covered = {}
     for c, p in run:
-        covered.setdefault(plan_class(p), c.name)
-    per_class = collections.Counter(plan_class(p) for _, _, _, p in launches)
-    lines = [f"{len(per_class)} product plan classes, {len(launches)} launches, {len(reps)} groups replayed, "
-             f"{len(HAND_CASES)} hand-written cases"]
-    lines += [f"  {plan_label(cls):32s} launches={count:4d}  covered by {covered.get(cls, 'NOTHING')}"
-              for cls, count in sorted(per_class.items())]
+        covered.setdefault(plan_variant(p), c.name)
+    per_variant = collections.Counter(plan_variant(la.plan) for la in runs)
+    lines += [f"  {variant_label(v):48s} launches={count:5d}  covered by {covered.get(v, 'NOTHING')}"
+              for v, count in sorted(per_variant.items())]
     report(request.config, lines)
-    assert set(per_class) <= set(covered), sorted(set(per_class) - set(covered))
+    assert set(per_variant) <= set(covered), sorted(set(per_variant) - set(covered))
 
     def has(pred):
         return any(pred(c, p) for c, p in run)
@@ -184,7 +130,7 @@ def test_every_product_plan_class_is_covered(request):
         ("SB = 1", lambda c, p: not p["resident"] and p["SB"] == 1),
         ("N = 256", lambda c, p: p["N"] == 256),
     ] if not has(pred)]
-    three_seg_n = {p["N"] for _, _, c, p in launches if len(c.segs) == 3}
+    three_seg_n = {la.plan["N"] for la in runs if len(la.case.segs) == 3}
     missing += [f"3-segment concat at N = {n}" for n in sorted(three_seg_n)
                 if not has(lambda c, p: len(c.segs) == 3 and p["N"] == n)]
     assert not missing, missing

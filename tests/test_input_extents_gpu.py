@@ -40,6 +40,7 @@ from tests._coarse_pool_inputs import epilogue_input
 from tests._coarse_view_inputs import seeded_lut
 from tests._depression_inputs import fill_case, smooth_case
 from tests._fence import FENCED_ARGS, Fenced, FencedStruct
+from tests._igemm_surface import gpu_tests_selected, product_representatives, surface_representatives
 from tests._hydrology_inputs import hydrology_case, smooth_field
 from tests._minecraft_inputs import planes as mc_planes
 from tests._post_inputs import field
@@ -233,7 +234,7 @@ def igemm_case(c: IR.Case, env):
 
 
 def igemm_cases() -> list:
-    reps = IP.product()[1] if _gpu_run[0] else []
+    reps = list(product_representatives()) + list(surface_representatives()) if _gpu_run[0] else []
     return [Case(f"tdx_igemm_run[{c.name}]", "tdx_igemm_run", functools.partial(igemm_case, c))
             for c in IP.HAND_CASES + reps]
 
@@ -863,7 +864,7 @@ def _synthetic(env, kind, h, w):
 # ========================================================================================================= tests
 def pytest_generate_tests(metafunc):
     if metafunc.function.__name__ == "test_inputs_are_read_inside_their_extent":
-        _gpu_run[0] = IP._gpu_tests_selected(metafunc.config)
+        _gpu_run[0] = gpu_tests_selected(metafunc.config)
         cases = CASES + igemm_cases()
         metafunc.parametrize("c", cases, ids=[c.name for c in cases])
 
