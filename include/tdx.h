@@ -288,6 +288,22 @@ int tdx_minecraft_readout(const float* elev, int32_t h, int32_t w, int32_t scale
                           float slope_div, float* elev_out, float* smooth_out, float* climate_out, int16_t* biome_out,
                           void* payload, void* stream);
 
+/* The terrain read-out of the generative evaluations (evaluation/base_consistency.py:34-72 `_decode_latents_to_terrain`,
+ * shared by base_diffusion.py and the infinite_consistency*.py drivers) for a batch of n images in one call.  Inputs
+ * in normalised units: residual [n][H][W] (the consistency decoder's output) and lowfreq [n][h][w], H = 8h, W = 8w.
+ * Per image, exactly as terrain_diffusion_b200/inference/postproc.py chains tdx_post_pad_extrapolate,
+ * tdx_resize_aa_axis, tdx_gaussian_blur and tdx_post_combine (bit for bit):
+ *   r = residual * residual_std + residual_mean,  l = lowfreq * lowfreq_std + lowfreq_mean   (fp32 mul, then add);
+ *   denoise != 0: l = gaussian_blur(resize(laplacian_decode(r, l, extrapolate), int size w), 11, sigma 5)
+ *                 (laplacian_denoise(sigma=5); the int size makes the SHORTER edge w, as torchvision does);
+ *   out = f(laplacian_decode(r, l, extrapolate)), f = sign(v) v^2 when signed_square != 0, else the identity.
+ * With denoise, W <= 8H (a wider image would be upsampled before the blur) and the denoised plane must exceed 5 x 5.
+ * scratch: DEVICE fp32, at least 2 * n * (H + 16) * (W + 16) elements (scratch_elems).  out [n][H][W]; neither out
+ * nor scratch may overlap the inputs or each other.  n <= 65535, H + 16 <= 65535. */
+int tdx_eval_terrain(const float* residual, const float* lowfreq, int32_t n, int32_t h, int32_t w, float residual_mean,
+                     float residual_std, float lowfreq_mean, float lowfreq_std, int32_t denoise, int32_t signed_square,
+                     float* out, float* scratch, int64_t scratch_elems, void* stream);
+
 /* Climate read-out (WorldPipeline._compute_climate, inference/world_pipeline.py:1314-1365).
  * tdx_lapse_rate = local_baseline_temperature_torch (inference/postprocessing.py:262-326) on the normalised coarse
  * planes: `coarse_elev_sqrt` is coarse channel 0 (signed square root of metres; e = max(0, c)^2 inside), `temp` channel

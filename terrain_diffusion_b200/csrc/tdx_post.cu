@@ -6,6 +6,7 @@
 // All arithmetic is written with explicitly rounded operations in the order of the CPU restatement (oracle/postproc.py,
 // pinned against the reference), so results agree to float32 round-off.  HBM-bound and tiny (a few hundred KB per call).
 #include "tdx_common.h"
+#include "tdx_post.cuh"
 #include "tdx_ptx.cuh"
 #include "tdx_upsample.cuh"
 
@@ -21,30 +22,15 @@ __global__ void post_normalize_kernel(const float* __restrict__ num, const float
   out[(long)y * w + x] = __fadd_rn(__fmul_rn(q, scale), offset);
 }
 
-// laplacian_encoder.py:6-40: rows are extrapolated first, then the columns of the row-padded tensor.
-__device__ __forceinline__ float row_padded(const float* x, int h, int w, int r, int c) {   // r in [-1, h], c in [0, w)
-  if (r >= 0 && r < h) return x[(long)r * w + c];
-  if (h == 1) return x[c];
-  if (r < 0) return __fsub_rn(__fmul_rn(2.0f, x[c]), x[(long)w + c]);
-  return __fsub_rn(__fmul_rn(2.0f, x[(long)(h - 1) * w + c]), x[(long)(h - 2) * w + c]);
-}
 __global__ void post_pad_extrapolate_kernel(const float* __restrict__ x, int h, int w, float* __restrict__ out) {
   pdl_launch_dependents();
   pdl_wait();
   const int ox = blockIdx.x * blockDim.x + threadIdx.x, oy = blockIdx.y;
   if (ox >= w + 2 || oy >= h + 2) return;
-  const int r = oy - 1, c = ox - 1;
-  float v;
-  if (c >= 0 && c < w) v = row_padded(x, h, w, r, c);
-  else if (w == 1) v = row_padded(x, h, w, r, 0);
-  else if (c < 0) v = __fsub_rn(__fmul_rn(2.0f, row_padded(x, h, w, r, 0)), row_padded(x, h, w, r, 1));
-  else v = __fsub_rn(__fmul_rn(2.0f, row_padded(x, h, w, r, w - 1)), row_padded(x, h, w, r, w - 2));
-  out[(long)oy * (w + 2) + ox] = v;
+  const auto ld = [&](int r, int c) { return x[(long)r * w + c]; };
+  out[(long)oy * (w + 2) + ox] = pad_extrapolate_at(ld, h, w, oy, ox);
 }
 
-// One axis of torch's interpolate(mode="bilinear", antialias=True) (ATen UpSampleKernel.cpp,
-// _compute_indices_min_size_weights_aa with the triangle filter): weights are normalised first, then accumulated in
-// tap order.  axis 1: out[y][i] over rows of x;  axis 0: out[i][x] over columns.
 __global__ void resize_aa_axis_kernel(const float* __restrict__ x, int h, int w, float* __restrict__ out, int out_size,
                                       int axis) {
   pdl_launch_dependents();
@@ -52,59 +38,16 @@ __global__ void resize_aa_axis_kernel(const float* __restrict__ x, int h, int w,
   const int ox = blockIdx.x * blockDim.x + threadIdx.x, oy = blockIdx.y;
   const int oh = axis == 0 ? out_size : h, ow = axis == 1 ? out_size : w;
   if (ox >= ow || oy >= oh) return;
-  const int in_size = axis == 1 ? w : h;
-  const int i = axis == 1 ? ox : oy;
-  const float scale = __fdiv_rn((float)in_size, (float)out_size);
-  const float support = scale >= 1.0f ? scale : 1.0f;
-  const float invscale = scale >= 1.0f ? __fdiv_rn(1.0f, scale) : 1.0f;
-  const float center = __fmul_rn(scale, (float)i + 0.5f);
-  int lo = (int)__fadd_rn(__fsub_rn(center, support), 0.5f);
-  lo = lo > 0 ? lo : 0;
-  int hi = (int)__fadd_rn(__fadd_rn(center, support), 0.5f);
-  hi = hi < in_size ? hi : in_size;
-  const int n = hi - lo;
-  auto weight = [&](int j) {
-    float t = __fmul_rn(__fadd_rn(__fsub_rn((float)(j + lo), center), 0.5f), invscale);
-    t = t < 0.f ? -t : t;
-    return t < 1.0f ? __fsub_rn(1.0f, t) : 0.0f;
-  };
-  float total = 0.f;
-  for (int j = 0; j < n; ++j) total = __fadd_rn(total, weight(j));
-  const long stride = axis == 1 ? 1 : w;
-  const float* src = axis == 1 ? x + (long)oy * w + lo : x + (long)lo * w + ox;
-  float acc = 0.f;
-  for (int j = 0; j < n; ++j) {
-    float wj = weight(j);
-    if (total != 0.f) wj = __fdiv_rn(wj, total);
-    const float term = __fmul_rn(src[(long)j * stride], wj);
-    acc = j == 0 ? term : __fadd_rn(acc, term);
-  }
-  out[(long)oy * ow + ox] = acc;
+  out[(long)oy * ow + ox] = resize_aa_at(x, h, w, out_size, axis, oy, ox);
 }
 
-struct BlurParams {
-  float k[32];
-  int ksize;
-};
-// torchvision gaussian_blur: reflect padding ksize/2, 2-D kernel = outer(k, k), taps accumulated row-major.
 __global__ void gaussian_blur_kernel(const float* __restrict__ x, int h, int w, float* __restrict__ out,
                                      const BlurParams bp) {
   pdl_launch_dependents();
   pdl_wait();
   const int ox = blockIdx.x * blockDim.x + threadIdx.x, oy = blockIdx.y;
   if (ox >= w || oy >= h) return;
-  const int p = bp.ksize / 2;
-  float acc = 0.f;
-  for (int dy = 0; dy < bp.ksize; ++dy) {
-    int yy = oy + dy - p;
-    yy = yy < 0 ? -yy : (yy >= h ? 2 * h - 2 - yy : yy);
-    for (int dx = 0; dx < bp.ksize; ++dx) {
-      int xx = ox + dx - p;
-      xx = xx < 0 ? -xx : (xx >= w ? 2 * w - 2 - xx : xx);
-      acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(bp.k[dy], bp.k[dx]), x[(long)yy * w + xx]));
-    }
-  }
-  out[(long)oy * w + ox] = acc;
+  out[(long)oy * w + ox] = gaussian_blur_at(x, h, w, bp, oy, ox);
 }
 
 __global__ void post_combine_kernel(const float* __restrict__ a, long a_pitch, const float* __restrict__ b, long b_pitch,
@@ -115,7 +58,7 @@ __global__ void post_combine_kernel(const float* __restrict__ a, long a_pitch, c
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
   if (x >= w || y >= h) return;
   float v = __fadd_rn(a[(long)y * a_pitch + x], b[(long)y * b_pitch + x]);
-  if (signed_square) v = v == 0.f ? 0.f : copysignf(__fmul_rn(v, v), v);   // sign(v) * v^2 (world_pipeline.py:1312)
+  if (signed_square) v = tdx::signed_square(v);
   if (out) out[(long)y * w + x] = v;
   if (out_i16) out_i16[(long)y * w + x] = elev_to_i16(v);
 }
@@ -307,17 +250,7 @@ extern "C" int tdx_gaussian_blur(const float* x, int32_t h, int32_t w, float* ou
   TDX_REQUIRE(sigma > 0.f, "gaussian_blur: sigma must be positive");
   TDX_REQUIRE(h > ksize / 2 && w > ksize / 2 && h <= 65535,
               "gaussian_blur: reflect padding of %d needs both dimensions larger than that (got %d x %d)", ksize / 2, h, w);
-  BlurParams bp;
-  bp.ksize = ksize;
-  // torchvision _get_gaussian_kernel1d in float32: taps on linspace(-(k-1)/2, (k-1)/2, k), normalised by their sum
-  const float half = (ksize - 1) * 0.5f;
-  float sum = 0.f;
-  for (int i = 0; i < ksize; ++i) {
-    const float t = (-half + (float)i) / sigma;
-    bp.k[i] = expf(-0.5f * (t * t));
-    sum += bp.k[i];
-  }
-  for (int i = 0; i < ksize; ++i) bp.k[i] /= sum;
+  const BlurParams bp = gaussian_blur_params(ksize, sigma);
   TDX_CHECK_CUDA(launch(gaussian_blur_kernel, dim3((w + 127) / 128, h), 128, 0, stream, x, (int)h, (int)w, out, bp));
   return TDX_OK;
 }
