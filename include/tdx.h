@@ -303,6 +303,20 @@ int tdx_minecraft_readout(const float* elev, int32_t h, int32_t w, int32_t scale
 int tdx_eval_terrain(const float* residual, const float* lowfreq, int32_t n, int32_t h, int32_t w, float residual_mean,
                      float residual_std, float lowfreq_mean, float lowfreq_std, int32_t denoise, int32_t signed_square,
                      float* out, float* scratch, int64_t scratch_elems, void* stream);
+/* The read-out of the decoder evaluations (evaluation/decoder_consistency.py:183-196, tiled_decoder_consistency.py:
+ * 185-196) for n planes in one call: laplacian_decode(residual * residual_std + residual_mean, lowfreq_padded,
+ * pre_padded=True).  residual [n][H][W] in normalised units, lowfreq_padded [n][h+2][w+2] (the low-frequency plane
+ * with its one-pixel border, used as is), H = 8h, W = 8w.  Per plane, exactly as terrain_diffusion_b200/inference/
+ * postproc.py chains tdx_resize_aa_axis (to (H + 16) x (W + 16), width pass first), the crop by 8 on every side and
+ * tdx_post_combine (bit for bit):
+ *   out = f(residual * residual_std + residual_mean + up)   (fp32 mul, add, add),
+ * f = sign(v) v^2 when signed_square != 0, else the identity.  crop 0: out is [n][H][W]; else out is the centre
+ * [n][crop][crop], origin ((H - crop) / 2, (W - crop) / 2), 1 <= crop <= min(H, W).  scratch: DEVICE fp32, at least
+ * n * (h + 2) * (W + 16) elements (scratch_elems); neither out nor scratch may overlap the inputs or each other.
+ * n <= 65535, H + 16 <= 65535. */
+int tdx_eval_padded_terrain(const float* residual, const float* lowfreq_padded, int32_t n, int32_t h, int32_t w,
+                            float residual_mean, float residual_std, int32_t signed_square, int32_t crop, float* out,
+                            float* scratch, int64_t scratch_elems, void* stream);
 
 /* Climate read-out (WorldPipeline._compute_climate, inference/world_pipeline.py:1314-1365).
  * tdx_lapse_rate = local_baseline_temperature_torch (inference/postprocessing.py:262-326) on the normalised coarse

@@ -153,6 +153,9 @@ def _declare(l: C.CDLL) -> None:
     l.tdx_eval_terrain.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float,
                                    C.c_float, C.c_float, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64,
                                    C.c_void_p]
+    l.tdx_eval_padded_terrain.restype = C.c_int
+    l.tdx_eval_padded_terrain.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float,
+                                          C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
     l.tdx_lapse_rate.restype = C.c_int
     l.tdx_lapse_rate.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_float,
                                  C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]

@@ -59,10 +59,25 @@ __global__ void eval_combine_kernel(const float* __restrict__ residual, float sc
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
   if (x >= W || y >= H) return;
   const long p = blockIdx.z;
-  const float r = __fadd_rn(__fmul_rn(residual[p * H * W + (long)y * W + x], scale), offset);
-  float v = __fadd_rn(r, up[p * up_plane + (long)(y + oi) * up_pitch + x + oj]);
-  if (signed_sq) v = signed_square(v);
-  out[p * out_plane + (long)y * W + x] = v;
+  out[p * out_plane + (long)y * W + x] = denorm_combine(residual[p * H * W + (long)y * W + x], scale, offset,
+                                                        up[p * up_plane + (long)(y + oi) * up_pitch + x + oj], signed_sq);
+}
+
+// The decoder evaluations' read-out of pre-padded low-frequency planes: out[p][y][x] over the [ch][cw] crop at (cy, cx)
+// = f(residual[p][cy + y][cx + x] * scale + offset + up[cy + y + 8][cx + x + 8]), where up is the height pass of the
+// (H + 16) x (W + 16) resize, evaluated here from the width pass tmp [lh][W + 16] (plane stride tmp_plane) only where
+// the crop reads it.
+__global__ void eval_padded_combine_kernel(const float* __restrict__ residual, float scale, float offset,
+                                           const float* __restrict__ tmp, long tmp_plane, int lh, int H, int W,
+                                           int cy, int cx, float* __restrict__ out, int ch, int cw, int signed_sq) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+  if (x >= cw || y >= ch) return;
+  const long p = blockIdx.z;
+  const float up = resize_aa_at(tmp + p * tmp_plane, lh, W + 16, H + 16, 0, cy + y + 8, cx + x + 8);
+  out[p * ch * cw + (long)y * cw + x] =
+      denorm_combine(residual[p * H * W + (long)(cy + y) * W + cx + x], scale, offset, up, signed_sq);
 }
 
 namespace {
@@ -198,5 +213,37 @@ extern "C" int tdx_eval_terrain(const float* residual, const float* lowfreq, int
   r.cur ^= 1;
   // ... then laplacian_decode(residual, denoised lowfreq, extrapolate=True)
   TDX_CHECK_CUDA(r.decode(residual, r.buf[r.cur], plane, nh, nw, 0, 1.f, 0.f, out, (long)H * W, signed_square));
+  return TDX_OK;
+}
+
+// The decoder evaluations' read-out (evaluation/decoder_consistency.py:183-196, tiled_decoder_consistency.py:185-196):
+// laplacian_decode(residual * std + mean, lowfreq_padded, pre_padded=True) (laplacian_encoder.py:93-132), whose low-
+// frequency plane arrives with its one-pixel border: resized to (H + 16) x (W + 16), cropped by pad_pixels = W / w = 8
+// on every side.  Then the optional signed square and centre crop.  Two launches over the whole batch: the width pass
+// into scratch, then the height pass fused with the combine and the crop.
+extern "C" int tdx_eval_padded_terrain(const float* residual, const float* lowfreq_padded, int32_t n, int32_t h,
+                                       int32_t w, float residual_mean, float residual_std, int32_t signed_square,
+                                       int32_t crop, float* out, float* scratch, int64_t scratch_elems, void* stream) {
+  TDX_REQUIRE(residual && lowfreq_padded && out && scratch, "eval_padded_terrain: null pointer");
+  TDX_REQUIRE(n >= 1 && n <= 65535, "eval_padded_terrain: batch of %d planes (1..65535)", n);
+  TDX_REQUIRE(h >= 1 && w >= 1 && 8 * (int64_t)h + 16 <= 65535 && w <= (1 << 24),
+              "eval_padded_terrain: bad low-frequency shape %d x %d (before its padding)", h, w);
+  const int H = 8 * h, W = 8 * w;
+  TDX_REQUIRE(crop >= 0 && crop <= H && crop <= W, "eval_padded_terrain: crop %d of a %d x %d plane", crop, H, W);
+  const int ch = crop ? crop : H, cw = crop ? crop : W;
+  const long tmp_plane = (long)(h + 2) * (W + 16);
+  const int64_t need = (int64_t)n * tmp_plane;
+  TDX_REQUIRE(scratch_elems >= need, "eval_padded_terrain: scratch holds %lld floats, %d planes of %d x %d need %lld",
+              (long long)scratch_elems, n, h, w, (long long)need);
+  const int64_t n_res = (int64_t)n * H * W, n_low = (int64_t)n * (h + 2) * (w + 2), n_out = (int64_t)n * ch * cw;
+  TDX_REQUIRE(!overlaps(out, n_out, residual, n_res) && !overlaps(out, n_out, lowfreq_padded, n_low) &&
+                  !overlaps(out, n_out, scratch, need) && !overlaps(scratch, need, residual, n_res) &&
+                  !overlaps(scratch, need, lowfreq_padded, n_low),
+              "eval_padded_terrain: out and scratch must not overlap each other or the inputs");
+  TDX_CHECK_CUDA(launch(eval_resize_kernel, dim3((W + 16 + 127) / 128, h + 2, n), 128, 0, stream, lowfreq_padded,
+                        (long)(h + 2) * (w + 2), h + 2, w + 2, scratch, tmp_plane, W + 16, 1));
+  TDX_CHECK_CUDA(launch(eval_padded_combine_kernel, dim3((cw + 127) / 128, ch, n), 128, 0, stream, residual,
+                        residual_std, residual_mean, (const float*)scratch, tmp_plane, h + 2, H, W, (H - ch) / 2,
+                        (W - cw) / 2, out, ch, cw, (int)signed_square));
   return TDX_OK;
 }

@@ -100,4 +100,12 @@ __device__ __forceinline__ float gaussian_blur_at(const float* __restrict__ x, i
 // sign(v) * v^2 (world_pipeline.py:1312)
 __device__ __forceinline__ float signed_square(float v) { return v == 0.f ? 0.f : copysignf(__fmul_rn(v, v), v); }
 
+// One element of laplacian_decode on a normalised residual: f(r * scale + offset + up), rounded as torch rounds
+// `residual * std + mean` (a multiply, then an add) followed by tdx_post_combine's add; f = sign(v) v^2 with signed_sq,
+// else the identity.
+__device__ __forceinline__ float denorm_combine(float r, float scale, float offset, float up, int signed_sq) {
+  const float v = __fadd_rn(__fadd_rn(__fmul_rn(r, scale), offset), up);
+  return signed_sq ? signed_square(v) : v;
+}
+
 }  // namespace tdx

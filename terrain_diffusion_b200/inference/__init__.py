@@ -14,6 +14,7 @@ from .pipeline import TerrainPipeline, WorldPipeline  # noqa: F401
 from .relief import get_relief_map  # noqa: F401
 from .hydrology import (d8_flow, fill_depressions_priority_flood, flow_accumulation,  # noqa: F401
                         plot_flow_indicator, smooth_river_bumps)
-from .evaluation import decode_latents_to_terrain, normalize_uint8_three_channel  # noqa: F401
+from .evaluation import (decode_latents_to_terrain, decoder_eval_terrain, normalize_uint8_three_channel,  # noqa: F401
+                         padded_terrain)
 from .multiphase import (build_timestep_ranges, infinite_diffusion_canvases, phase_step_ranges,  # noqa: F401
                          sample_infinite_diffusion)

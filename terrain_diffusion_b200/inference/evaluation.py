@@ -13,12 +13,18 @@ the same positional arguments, so a driver only swaps its import, and runs
 
 Nothing is copied to the host between the samples and the terrain.  `normalize_uint8_three_channel` is the drivers'
 `_normalize_uint8_three_channel`, as torch ops on the samples' device.
+
+The decoder evaluations (evaluation/decoder_consistency.py and tiled_decoder_consistency.py) measure the decoder
+itself on the dataset's residuals: `decoder_eval_terrain` is one batch of their loop, the tiled two-step TrigFlow decode
+as one fused program per step and the read-out of the generated and the real residual against the pre-padded
+low-frequency plane as one `padded_terrain` call (tdx_eval_padded_terrain).
 """
 from __future__ import annotations
 
 import math
 from typing import Optional
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -57,10 +63,10 @@ def _stats(val_dataset) -> tuple:
     return tuple(getattr(base, a) for a in DATASET_ATTRS)
 
 
-def _scalar(v, name: str) -> float:
+def _scalar(v, name: str, fn: str = "decode_latents_to_terrain") -> float:
     t = torch.as_tensor(v)
     if t.numel() != 1:
-        raise ValueError(f"decode_latents_to_terrain: {name} must be a scalar, got shape {tuple(t.shape)}")
+        raise ValueError(f"{fn}: {name} must be a scalar, got shape {tuple(t.shape)}")
     return float(t.reshape(()))
 
 
@@ -165,6 +171,124 @@ def decode_latents_to_terrain(samples: torch.Tensor, val_dataset, decoder_model,
     denoise = not disable_laplacian_denoising
     terrain = eval_terrain(residual, lowfreq.float().contiguous(), residual_mean, residual_std, denoise, signed_square)
     return terrain[:, None]
+
+
+def padded_terrain(residual: torch.Tensor, lowfreq_padded: torch.Tensor, residual_mean: float, residual_std: float,
+                   signed_square: bool = True, crop: Optional[int] = None) -> torch.Tensor:
+    """The decoder evaluations' batched read-out (tdx_eval_padded_terrain): residual [B, H, W] in normalised units and
+    the pre-padded low-frequency planes [B, h + 2, w + 2], CUDA fp32, H = 8h, W = 8w -> terrain [B, H, W]:
+    laplacian_decode(residual * residual_std + residual_mean, lowfreq_padded, pre_padded=True), optionally followed by
+    sign(x) x^2, and reduced to the centre crop x crop when `crop` is given."""
+    ok = all(isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float32 and t.dim() == 3
+             for t in (residual, lowfreq_padded))
+    if not ok or residual.device != lowfreq_padded.device:
+        raise L.TdxError("padded_terrain: residual and lowfreq_padded must be CUDA float32 [B, H, W] / [B, h+2, w+2] "
+                         "tensors on one device (the read-out has no CPU path)")
+    b, hp, wp = lowfreq_padded.shape
+    h, w = hp - 2, wp - 2
+    if h < 1 or w < 1 or tuple(residual.shape) != (b, 8 * h, 8 * w):
+        raise ValueError(f"padded_terrain: residual is {tuple(residual.shape)} and lowfreq_padded "
+                         f"{tuple(lowfreq_padded.shape)}; the read-out takes [B, 8h, 8w] with [B, h+2, w+2], h, w >= 1")
+    H, W = 8 * h, 8 * w
+    c = 0 if crop is None else int(crop)
+    if crop is not None and not 1 <= c <= min(H, W):
+        raise ValueError(f"padded_terrain: crop {crop} of a {H}x{W} plane (1..{min(H, W)})")
+    residual, lowfreq_padded = residual.contiguous(), lowfreq_padded.contiguous()
+    out = torch.empty((b, c or H, c or W), dtype=torch.float32, device=residual.device)
+    n_scratch = b * (h + 2) * (W + 16)
+    scratch = torch.empty((n_scratch,), dtype=torch.float32, device=residual.device)
+    L.call(L.lib().tdx_eval_padded_terrain, out.device, residual.data_ptr(), lowfreq_padded.data_ptr(), b, h, w,
+           float(residual_mean), float(residual_std), int(bool(signed_square)), c, out.data_ptr(), scratch.data_ptr(),
+           n_scratch)
+    return out
+
+
+def decoder_eval_times(scheduler, intermediate_sigma: float, sigma_data: float) -> list:
+    """The TrigFlow times of the decoder evaluations as the drivers form them (decoder_consistency.py:115-119): numpy's
+    atan of the scheduler's sigma_0 / sigma_data (fp32, as the sigma table is), then, when intermediate_sigma > 0, the
+    float64 atan(intermediate_sigma / sigma_data); both as the fp32 values the model sees."""
+    ts = [torch.as_tensor(np.arctan(torch.as_tensor(scheduler.sigmas[0] / sigma_data).numpy()))]
+    if intermediate_sigma > 0:
+        ts.append(torch.as_tensor(np.arctan(intermediate_sigma / sigma_data)))
+    return [float(t.to(torch.float32)) for t in ts]
+
+
+@torch.no_grad()
+def decoder_eval_terrain(model, scheduler, images: torch.Tensor, lowfreq_padded: torch.Tensor, cond_img: torch.Tensor,
+                         generator: Optional[torch.Generator], *, residual_mean, residual_std, sigma_data: float = 0.5,
+                         tile_size: int = 512, tile_stride: Optional[int] = None, intermediate_sigma: float = 0.065,
+                         crop_size: Optional[int] = None, tile_batch: Optional[int] = None) -> tuple:
+    """One batch of the decoder evaluations (evaluation/decoder_consistency.py:131-196 and tiled_decoder_consistency.py:
+    135-196) on the device: the dataset's images [B, 1, S, S] (residual * sigma_data), lowfreq_padded [B, 1, S/8 + 2,
+    S/8 + 2] and cond_img [B, C, S, S] -> (output_full, images_full), the generated and the real terrain in metres,
+    CUDA fp32 [B, 1, S, S], or [B, 1, crop_size, crop_size] for the centre crop.  The drivers' metric then takes
+    normalize_uint8_three_channel of each.
+
+    Tiles of tile_size start at k * tile_stride (default tile_size // 2) for k in range((S - T) // stride + 1) on both
+    axes.  Every tile runs the drivers' two-step TrigFlow loop, one step at atan(sigma_0 / sigma_data) and one at
+    atan(intermediate_sigma / sigma_data) (only the first when intermediate_sigma <= 0), each from a fresh
+    torch.randn((B, 1, T, T), generator=generator) drawn on the generator's device (images' device for None) in the
+    drivers' order, tiles row-major, then steps; all draws happen before the first solve, and leave the generator
+    where the drivers leave it.  Each step of `tile_batch` tiles (default: all) with all B images is one fused
+    consistency program.  The tiles are blended with the linear window (_get_weights) in row-major order and divided
+    by sigma_data; then the generated and the real residual (images / sigma_data) go through ONE padded_terrain call
+    (de-normalisation, pre-padded laplacian_decode, signed square, crop).
+
+    ValueError / TdxError before any device work for images that are not square CUDA [B, 1, S, S] tensors with
+    S a multiple of 8, inputs whose shapes disagree, or a crop larger than the image.  A tile geometry that leaves
+    pixels uncovered (T > S, stride > T, (S - T) % stride != 0 or T < 2) is a ValueError; the drivers divide 0 by 0
+    there and hand NaN to the metric, the only place this function does not do what they do."""
+    if not all(isinstance(t, torch.Tensor) and t.dim() == 4 for t in (images, lowfreq_padded, cond_img)):
+        raise ValueError("decoder_eval_terrain: images, lowfreq_padded and cond_img must be [B, C, H, W] tensors")
+    B, C, S, S2 = images.shape
+    if B < 1 or C != 1 or S != S2 or S < 8 or S % 8:
+        raise ValueError(f"decoder_eval_terrain: images are {tuple(images.shape)}; the drivers decode square "
+                         f"[B, 1, S, S] residuals with S a non-zero multiple of 8")
+    if tuple(lowfreq_padded.shape) != (B, 1, S // 8 + 2, S // 8 + 2):
+        raise ValueError(f"decoder_eval_terrain: lowfreq_padded is {tuple(lowfreq_padded.shape)}; {S}x{S} images "
+                         f"need {(B, 1, S // 8 + 2, S // 8 + 2)}")
+    if cond_img.shape[0] != B or tuple(cond_img.shape[-2:]) != (S, S):
+        raise ValueError(f"decoder_eval_terrain: cond_img is {tuple(cond_img.shape)}; it must be [{B}, C, {S}, {S}]")
+    T = int(tile_size)
+    stride = T // 2 if tile_stride is None else int(tile_stride)
+    if T < 2 or T > S or stride < 1 or stride > T or (S - T) % stride:
+        raise ValueError(f"decoder_eval_terrain: tiles of {T} at stride {stride} leave pixels of the {S}x{S} image "
+                         "uncovered (the drivers would divide 0 by 0 there)")
+    if crop_size is not None and not 1 <= int(crop_size) <= S:
+        raise ValueError(f"decoder_eval_terrain: crop_size {crop_size} of a {S}x{S} image")
+    if tile_batch is not None and int(tile_batch) < 1:
+        raise ValueError(f"decoder_eval_terrain: tile_batch must be >= 1, got {tile_batch}")
+    residual_mean = _scalar(residual_mean, "residual_mean", "decoder_eval_terrain")
+    residual_std = _scalar(residual_std, "residual_std", "decoder_eval_terrain")
+    device = images.device
+    if not images.is_cuda or lowfreq_padded.device != device or cond_img.device != device:
+        raise L.TdxError(f"decoder_eval_terrain: images, lowfreq_padded and cond_img must be on one CUDA device (there "
+                         f"is no CPU path); got {images.device}, {lowfreq_padded.device}, {cond_img.device}")
+
+    sigma_data = float(sigma_data)
+    ts = decoder_eval_times(scheduler, float(intermediate_sigma), sigma_data)
+    n_tiles = (S - T) // stride + 1
+    tiles = [(i * stride, j * stride, i * n_tiles + j) for i in range(n_tiles) for j in range(n_tiles)]
+    gen_dev = generator.device if generator is not None else device
+    noise = [[torch.randn((B, C, T, T), generator=generator, device=gen_dev) for _ in ts] for _ in tiles]
+    cond = cond_img.float()
+    window = _window(None, T, device)
+
+    def run_group(chunk):
+        ct = _gather(cond, chunk, T)
+        sample = None
+        for k, t in enumerate(ts):
+            zt = torch.cat([noise[q][k] for _, _, q in chunk], dim=0).to(device)
+            x = zt if k == 0 else trig_mix(sample, zt, math.cos(t), math.sin(t) * sigma_data)
+            solve = get_consistency_solve(model, zt.shape[0], T, T, t, sigma_data, from_unit_noise=k == 0)
+            sample = solve.run(x, ct)
+        return sample
+
+    output = _blend_tiles(tiles, tile_batch, B, C, S, S, window, run_group, sigma_data)
+    residual = torch.cat([output[:, 0], images[:, 0].float() / sigma_data])
+    lowfreq = lowfreq_padded[:, 0].float()
+    terrain = padded_terrain(residual, torch.cat([lowfreq, lowfreq]), residual_mean, residual_std, True, crop_size)
+    return terrain[:B, None], terrain[B:, None]
 
 
 def normalize_uint8_three_channel(images: torch.Tensor) -> torch.Tensor:
