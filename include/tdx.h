@@ -87,6 +87,12 @@ typedef struct TdxIgemmDesc {
    * the residual to recompute it.  Both may be NULL. */
   float* rms_out;
   const float* resid_inv;
+  /* Forced split-K factor (0: the library chooses).  With n_per_item, a forced value fixes the launch's item shape, so
+   * every image of the launch is summed in the same order whatever n_img is (batch-invariant plans: pass the shape
+   * the library picks for the same descriptor at n_img = 1).  A launch whose images do not all fit the
+   * device at a forced ksplit > 1 is issued as several launches over consecutive image ranges. */
+  int32_t ksplit;
+  int32_t _pad;
 } TdxIgemmDesc;
 
 /* Output channels per work item (64/128/192/256) the library prefers for this launch shape: balances the MMA issue
@@ -230,6 +236,13 @@ int tdx_window_to_cond(float* out, const float* packed, int32_t n_img, int32_t p
 int tdx_coarse_epilogue(float* out, const float* x, const float* means, const float* stds, const float* w,
                         int32_t n_img, int32_t size, int32_t pool, int32_t elev_mode, int32_t p5_mode, float sigma_data,
                         void* stream);
+/* Coarse-stage solve inputs for n_img windows in one launch (world_pipeline.py:921-933): per channel c < 5 and image,
+ * cond = cos_t[c] * ((map - means[c]) / stds[c]) + sin_t[c] * cond_noise, and sample[6 channels] = sample_noise * sigma0,
+ * each op rounded in fp32 in that order.  map, cond_noise, cond [n_img][5][plane]; sample_noise, sample
+ * [n_img][6][plane]; means, stds, cos_t, sin_t: 5 floats each on the device. */
+int tdx_coarse_condition(float* cond, float* sample, const float* map, const float* cond_noise,
+                         const float* sample_noise, const float* means, const float* stds, const float* cos_t,
+                         const float* sin_t, float sigma0, int32_t n_img, int64_t plane, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Elevation read-out (WorldPipeline._compute_elev, inference/world_pipeline.py:1277-1313): the reference normalises
@@ -564,6 +577,15 @@ int tdx_synthetic_map(const double* tables, int32_t n_knots, const int32_t* seed
                       const float* scalars, int64_t i0, int64_t j0, int32_t h, int32_t w, const float* input,
                       int32_t mode, const float* const* imp_values, const int64_t* imp_boxes, const float* imp_defaults,
                       uint32_t imp_has_default, float* out, void* stream);
+
+/* tdx_synthetic_map over n_img (1..TDX_SYNTH_MAX_IMAGES) windows of the same h x w at origins (HOST int64 [n_img][2]:
+ * i0, j0) into out [n_img][5][h][w], with the generators' noise (no input): every window is bit-identical to its own
+ * tdx_synthetic_map call.  mode: TDX_SYNTH_FINALIZE, TDX_SYNTH_SQRT0, TDX_SYNTH_IMPORT. */
+#define TDX_SYNTH_MAX_IMAGES 16
+int tdx_synthetic_maps(const double* tables, int32_t n_knots, const int32_t* seeds, const float* frequency,
+                       const float* scalars, int32_t n_img, const int64_t* origins, int32_t h, int32_t w, int32_t mode,
+                       const float* const* imp_values, const int64_t* imp_boxes, const float* imp_defaults,
+                       uint32_t imp_has_default, float* out, void* stream);
 
 #ifdef __cplusplus
 }

@@ -23,7 +23,8 @@ class TdxIgemmDesc(C.Structure):
         ("b_packed", C.c_void_p), ("c_out", C.c_int32), ("n_per_item", C.c_int32), ("n_img", C.c_int32),
         ("height", C.c_int32), ("width", C.c_int32), ("epi_flags", C.c_int32), ("cvec", C.c_void_p), ("resid", C.c_void_p),
         ("resid_spatial", C.c_int32), ("resid_pnorm", C.c_int32), ("resid_scale", C.c_float), ("clip", C.c_float),
-        ("out", TdxOutSpec * 3), ("rms_out", C.c_void_p), ("resid_inv", C.c_void_p),
+        ("out", TdxOutSpec * 3), ("rms_out", C.c_void_p), ("resid_inv", C.c_void_p), ("ksplit", C.c_int32),
+        ("_pad", C.c_int32),
     ]
 
 
@@ -96,6 +97,8 @@ def _declare(l: C.CDLL) -> None:
     l.tdx_debug_igemm_plan.restype = None
     l.tdx_debug_igemm_plan.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32),
                                        C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32)]
+    l.tdx_debug_igemm_launch_shape.restype = C.c_int
+    l.tdx_debug_igemm_launch_shape.argtypes = [C.POINTER(TdxIgemmDesc), C.POINTER(C.c_int32)]
     l.tdx_abi_sizeof.restype = C.c_int
     l.tdx_abi_sizeof.argtypes = [C.c_int]
     for i, st in enumerate(ABI_STRUCTS):
@@ -197,6 +200,10 @@ def _declare(l: C.CDLL) -> None:
     l.tdx_synthetic_map.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
                                     C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_uint32, C.c_void_p, C.c_void_p]
+    l.tdx_synthetic_maps.restype = C.c_int
+    l.tdx_synthetic_maps.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                     C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
+                                     C.c_void_p, C.c_void_p]
     l.tdx_flow_d8.restype = C.c_int
     l.tdx_flow_d8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -223,6 +230,9 @@ def _declare(l: C.CDLL) -> None:
     l.tdx_noise_patches.argtypes = [C.c_uint64, C.c_int32, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int32,
                                     C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64,
                                     C.c_void_p]
+    l.tdx_coarse_condition.restype = C.c_int
+    l.tdx_coarse_condition.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int32, C.c_int64, C.c_void_p]
     l.tdx_noise_patches_workspace_bytes.restype = C.c_int64
     l.tdx_noise_patches_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     l.tdx_standard_normal.restype = C.c_int
@@ -297,3 +307,10 @@ def igemm_choose_n(c_out: int, n_img: int, height: int, width: int, segs) -> int
     ch = (C.c_int32 * 3)(*[c for c, _ in segs], *([0] * (3 - len(segs))))
     tp = (C.c_int32 * 3)(*[t for _, t in segs], *([0] * (3 - len(segs))))
     return int(lib().tdx_igemm_choose_n(c_out, n_img, height, width, ch, tp, len(segs)))
+
+
+def igemm_launch_shape(desc: TdxIgemmDesc) -> tuple:
+    """(output channels per work item, split-K factor) a launch of `desc` uses (its forced ksplit, if any)."""
+    shape = (C.c_int32 * 2)()
+    check(lib().tdx_debug_igemm_launch_shape(C.byref(desc), shape))
+    return int(shape[0]), int(shape[1])

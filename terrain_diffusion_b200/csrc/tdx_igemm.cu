@@ -992,9 +992,12 @@ static int max_active_clusters(int csize) {
 //     `ks` CTAs of a cluster, which reduce-scatter fp32 partial sums through L2 (each part then finalises N/ks columns,
 //     so N/ks must be a multiple of the epilogue's 32-column chunk);
 //   * pixel-norm layers exchange statistics inside a cluster, so all nsplit*ks CTAs of an M tile share one (<= 8).
+//   A forced split-K factor (batch-invariant plans) is taken as it is, whatever the number of M tiles: the launch path
+//   then runs the images in as many launches as the one-item-per-CTA rule needs (igemm_launch).
 struct ItemShape { int ncta, resident, sa, sb, ksplit; };
 
-static ItemShape choose_item_shape(int cout, int tiles, int stages, int chunks, int forced_n, bool norm) {
+static ItemShape choose_item_shape(int cout, int tiles, int stages, int chunks, int forced_n, bool norm,
+                                   int forced_ks = 0) {
   if (forced_n && (forced_n > cout || cout % forced_n)) forced_n = 0;
   double best = 1e30;
   ItemShape bs = {64, 0, kSA, 2, 1};
@@ -1009,11 +1012,12 @@ static ItemShape choose_item_shape(int cout, int tiles, int stages, int chunks, 
     const int ring_budget = free_bytes - sa * kAStageBytes;
     const long items = (long)tiles * nsplit;
     for (int ks = 1; ks <= 8; ++ks) {
+      if (forced_ks && ks != forced_ks) continue;
       const int csize = ks * ((norm && nsplit > 1) ? nsplit : 1);
       if (ks > 1) {
         if (n % (kChunk * ks) || ks > stages || csize > kMaxSplit) continue;
-        if (items * ks > (long)max_active_clusters(csize) * csize) continue;   // one item per CTA, all resident
-        if ((size_t)items * (ks - 1) * n * 512 > kWsBytes) continue;
+        if (!forced_ks && items * ks > (long)max_active_clusters(csize) * csize) continue;   // one item per CTA, all resident
+        if (!forced_ks && (size_t)items * (ks - 1) * n * 512 > kWsBytes) continue;
       }
       const int my_stages = (stages + ks - 1) / ks;
       const int my_chunks = (chunks + ks - 1) / ks + (ks > 1 ? 1 : 0);
@@ -1047,7 +1051,70 @@ static ItemShape choose_item_shape(int cout, int tiles, int stages, int chunks, 
   return bs;
 }
 
+// Images per launch of a split-K descriptor: every CTA holds one item and the fp32 partial sums fit the workspace.
+static int split_images_per_launch(const TdxIgemmDesc& d, const ItemShape& shp, bool norm, int tiles_per_img) {
+  const int nsplit = d.c_out / shp.ncta;
+  const int csize = shp.ksplit * ((norm && nsplit > 1) ? nsplit : 1);
+  const long per_img = (long)tiles_per_img * nsplit * shp.ksplit;
+  const long by_sms = (long)max_active_clusters(csize) * csize / per_img;
+  const long by_ws = (long)(kWsBytes / ((size_t)tiles_per_img * nsplit * (shp.ksplit - 1) * shp.ncta * 512));
+  return (int)(by_sms < by_ws ? by_sms : by_ws);
+}
+
+// Descriptor of images [i0, i0 + n) of `d`: every tensor of a launch is image-major.
+static TdxIgemmDesc image_slice(const TdxIgemmDesc& d, int i0, int n) {
+  TdxIgemmDesc s = d;
+  const size_t plane = (size_t)d.height * d.width;
+  auto at = [](const void* ptr, size_t bytes) -> const uint8_t* {
+    return ptr ? reinterpret_cast<const uint8_t*>(ptr) + bytes : nullptr;
+  };
+  auto scaled = [&](int spatial) { return spatial == TDX_SP_DOWN2 ? plane / 4 : (spatial == TDX_SP_UP2 ? plane * 4 : plane); };
+  for (int k = 0; k < d.n_seg; ++k) s.a_ptr[k] = at(d.a_ptr[k], (size_t)i0 * d.a_channels[k] * plane * 2);
+  // the residual is read at the inverse of an output's resampling ("UP2": it is at half resolution)
+  const size_t rplane = d.resid_spatial == TDX_SP_UP2 ? plane / 4 : (d.resid_spatial == TDX_SP_DOWN2 ? plane * 4 : plane);
+  s.resid = at(d.resid, (size_t)i0 * d.c_out * rplane * 2);
+  s.resid_inv = reinterpret_cast<const float*>(at(d.resid_inv, (size_t)i0 * rplane * 4));
+  s.cvec = reinterpret_cast<const float*>(at(d.cvec, (size_t)i0 * d.c_out * 4));
+  s.rms_out = const_cast<float*>(reinterpret_cast<const float*>(at(d.rms_out, (size_t)i0 * plane * 4)));
+  for (int o = 0; o < 3; ++o)
+    if (d.out[o].kind != TDX_OUT_NONE)
+      s.out[o].ptr = const_cast<uint8_t*>(at(d.out[o].ptr, (size_t)i0 * d.c_out * scaled(d.out[o].spatial) * 2));
+  s.n_img = n;
+  return s;
+}
+
+static int igemm_launch_one(const TdxIgemmDesc& d, const CUtensorMap* tms, cudaStream_t stream);
+
 int igemm_launch(const TdxIgemmDesc& d, const CUtensorMap* tms, cudaStream_t stream) {
+  if (d.ksplit > 1) {
+    int chunks = 0, stages = 0;
+    for (int s = 0; s < d.n_seg; ++s) {
+      chunks += d.a_channels[s] / 64;
+      stages += (d.a_channels[s] / 64) * d.a_taps[s];
+    }
+    const int per_img = ((d.width + kTileW - 1) / kTileW) * ((d.height + kTileH - 1) / kTileH);
+    const bool norm = needs_norm(d);
+    const ItemShape shp = choose_item_shape(d.c_out, per_img * d.n_img, stages, chunks, d.n_per_item, norm, d.ksplit);
+    const int step = split_images_per_launch(d, shp, norm, per_img);
+    TDX_REQUIRE(step >= 1, "igemm: ksplit=%d does not fit one %dx%d image on this device", d.ksplit, d.height, d.width);
+    if (step < d.n_img) {
+      for (int i0 = 0; i0 < d.n_img; i0 += step) {
+        const TdxIgemmDesc s = image_slice(d, i0, d.n_img - i0 < step ? d.n_img - i0 : step);
+        CUtensorMap stm[3];
+        for (int k = 0; k < s.n_seg; ++k) {
+          int rc = make_act_tensor_map(&stm[k], s.a_ptr[k], s.n_img, s.a_channels[k], s.height, s.width);
+          if (rc != TDX_OK) return rc;
+        }
+        int rc = igemm_launch_one(s, stm, stream);
+        if (rc != TDX_OK) return rc;
+      }
+      return TDX_OK;
+    }
+  }
+  return igemm_launch_one(d, tms, stream);
+}
+
+static int igemm_launch_one(const TdxIgemmDesc& d, const CUtensorMap* tms, cudaStream_t stream) {
   IgemmParams p;
   memset(&p, 0, sizeof(p));
   p.nseg = d.n_seg;
@@ -1069,7 +1136,7 @@ int igemm_launch(const TdxIgemmDesc& d, const CUtensorMap* tms, cudaStream_t str
   p.tiles_y = (d.height + kTileH - 1) / kTileH;
   const int tiles = p.tiles_x * p.tiles_y * d.n_img;
   const bool norm = needs_norm(d);
-  const ItemShape shp = choose_item_shape(d.c_out, tiles, p.stages_per_item, chunks, d.n_per_item, norm);
+  const ItemShape shp = choose_item_shape(d.c_out, tiles, p.stages_per_item, chunks, d.n_per_item, norm, d.ksplit);
   p.ncta = shp.ncta;
   p.resident = shp.resident;
   p.SA = shp.sa;
@@ -1146,6 +1213,16 @@ int igemm_validate(const TdxIgemmDesc& d) {
   TDX_REQUIRE(d.n_per_item >= 64 && d.n_per_item <= 256 && d.n_per_item % 64 == 0 && d.c_out % d.n_per_item == 0,
               "igemm: n_per_item=%d must be 64/128/192/256 and divide c_out=%d (use tdx_igemm_choose_n)", d.n_per_item,
               d.c_out);
+  if (d.ksplit) {
+    int stages = 0;
+    for (int s = 0; s < d.n_seg; ++s) stages += (d.a_channels[s] / 64) * d.a_taps[s];
+    const int nsplit = d.c_out / d.n_per_item;
+    const int csize = d.ksplit * ((needs_norm(d) && nsplit > 1) ? nsplit : 1);
+    TDX_REQUIRE(d.ksplit >= 1 && d.ksplit <= 8 && d.n_per_item % (kChunk * d.ksplit) == 0 && d.ksplit <= stages &&
+                    csize <= kMaxSplit,
+                "igemm: forced ksplit=%d needs 1..8, <= the %d K stages, n_per_item=%d a multiple of %d * ksplit and "
+                "a cluster of at most %d CTAs", d.ksplit, stages, d.n_per_item, kChunk, kMaxSplit);
+  }
   TDX_REQUIRE((unsigned long long)d.n_img * (d.c_out / 8) * d.height * d.width * 4ull < (1ull << 32),
               "igemm: tensor of %d x %d x %d x %d exceeds the 32-bit element offsets of the epilogue", d.n_img, d.c_out,
               d.height, d.width);
@@ -1213,6 +1290,34 @@ extern "C" void tdx_debug_igemm_plan(int32_t c_out, int32_t n_img, int32_t heigh
   const int tiles = ((width + tdx::kTileW - 1) / tdx::kTileW) * ((height + tdx::kTileH - 1) / tdx::kTileH) * n_img;
   tdx::ItemShape shp = tdx::choose_item_shape(c_out, tiles, stages, chunks, n_per_item, needs_norm != 0);
   out4[0] = shp.ncta; out4[1] = shp.ksplit; out4[2] = shp.resident; out4[3] = shp.sb;
+}
+
+// The item shape a launch of `desc` uses, without device work: shape[0] = output channels per work item, shape[1] = the
+// split-K factor (desc->ksplit when forced, else the library's choice for desc->n_img).  Batch-invariant plans ask it
+// for the descriptor at n_img = 1 and force the answer (models/plan.py).
+extern "C" int tdx_debug_igemm_launch_shape(const TdxIgemmDesc* desc, int32_t* shape) {
+  TDX_REQUIRE(desc && shape, "igemm_launch_shape: null argument");
+  const TdxIgemmDesc& d = *desc;
+  // the fields the shape depends on (no pointers: a planner may ask before it has buffers)
+  TDX_REQUIRE(d.n_seg >= 1 && d.n_seg <= 3, "igemm_launch_shape: n_seg=%d not in 1..3", d.n_seg);
+  int stages = 0, chunks = 0;
+  for (int s = 0; s < d.n_seg; ++s) {
+    TDX_REQUIRE(d.a_channels[s] > 0 && d.a_channels[s] % 64 == 0 && (d.a_taps[s] == 9 || d.a_taps[s] == 1),
+                "igemm_launch_shape: segment %d has %d channels, %d taps", s, d.a_channels[s], d.a_taps[s]);
+    stages += (d.a_channels[s] / 64) * d.a_taps[s];
+    chunks += d.a_channels[s] / 64;
+  }
+  TDX_REQUIRE(d.c_out >= 64 && d.c_out <= 2048 && d.c_out % 64 == 0 && d.n_per_item >= 64 && d.n_per_item <= 256 &&
+                  d.n_per_item % 64 == 0 && d.c_out % d.n_per_item == 0 && d.ksplit >= 0 && d.ksplit <= 8 &&
+                  d.n_img >= 1 && d.height >= 8 && d.width >= 8,
+              "igemm_launch_shape: bad shape c_out=%d n_per_item=%d ksplit=%d n=%d h=%d w=%d", d.c_out, d.n_per_item,
+              d.ksplit, d.n_img, d.height, d.width);
+  const int tiles = ((d.width + tdx::kTileW - 1) / tdx::kTileW) * ((d.height + tdx::kTileH - 1) / tdx::kTileH) * d.n_img;
+  const tdx::ItemShape shp = tdx::choose_item_shape(d.c_out, tiles, stages, chunks, d.n_per_item, tdx::needs_norm(d),
+                                                    d.ksplit);
+  shape[0] = shp.ncta;
+  shape[1] = shp.ksplit;
+  return TDX_OK;
 }
 
 extern "C" int64_t tdx_igemm_packed_weight_elems(const int32_t* a_channels, const int32_t* a_taps, int32_t n_seg,

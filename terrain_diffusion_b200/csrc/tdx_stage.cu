@@ -127,9 +127,48 @@ coarse_epilogue_kernel(float* out, const float* x, const float* means, const flo
   }
 }
 
+// Coarse solve inputs (world_pipeline.py:921-933): blockIdx.y = channel (0..5, 5 = only the sample's last channel),
+// blockIdx.z = image.  Every op is rounded on its own, in the order of the torch ops it replaces.
+constexpr int COARSE_MAP_CH = 5;
+
+__global__ void coarse_condition_kernel(float* cond, float* sample, const float* map, const float* cond_noise,
+                                        const float* sample_noise, const float* means, const float* stds,
+                                        const float* cos_t, const float* sin_t, float sigma0, int64_t plane) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int c = blockIdx.y, img = blockIdx.z;
+  const size_t ci = ((size_t)img * COARSE_MAP_CH + c) * plane, si = ((size_t)img * COARSE_CH + c) * plane;
+  const bool has_cond = c < COARSE_MAP_CH;
+  const float mean = has_cond ? means[c] : 0.f, sd = has_cond ? stds[c] : 1.f;
+  const float ct = has_cond ? cos_t[c] : 0.f, st = has_cond ? sin_t[c] : 0.f;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < plane; i += stride) {
+    if (has_cond) {
+      const float m = __fdiv_rn(__fsub_rn(map[ci + i], mean), sd);
+      cond[ci + i] = __fadd_rn(__fmul_rn(ct, m), __fmul_rn(st, cond_noise[ci + i]));
+    }
+    sample[si + i] = __fmul_rn(sample_noise[si + i], sigma0);
+  }
+}
+
 }  // namespace tdx
 
 using namespace tdx;
+
+extern "C" int tdx_coarse_condition(float* cond, float* sample, const float* map, const float* cond_noise,
+                                    const float* sample_noise, const float* means, const float* stds,
+                                    const float* cos_t, const float* sin_t, float sigma0, int32_t n_img, int64_t plane,
+                                    void* stream) {
+  TDX_REQUIRE(cond && sample && map && cond_noise && sample_noise && means && stds && cos_t && sin_t,
+              "coarse_condition: null pointer");
+  TDX_REQUIRE(n_img >= 1 && n_img <= 65535 && plane >= 1 && plane <= (1LL << 31),
+              "coarse_condition: bad shape (need 1 <= n_img <= 65535, 1 <= plane <= 2^31)");
+  int bx = (int)((plane + 255) / 256);
+  if (bx > 1024) bx = 1024;
+  TDX_CHECK_CUDA(launch(coarse_condition_kernel, dim3(bx, COARSE_CH, n_img), 256, 0, stream, cond, sample, map,
+                        cond_noise, sample_noise, means, stds, cos_t, sin_t, sigma0, plane));
+  return TDX_OK;
+}
 
 extern "C" int tdx_trig_mix(float* out, const float* sample, const float* noise, int64_t numel, float a, float b,
                             void* stream) {

@@ -204,9 +204,14 @@ __device__ __forceinline__ void finalize(float v[kFields], const SynthParams& p)
   v[4] = pcv;
 }
 
-// one thread per cell (r, c) of the [5, h, w] window at x = arange(j0, j0 + w)[c], y = arange(i0, i0 + h)[r]
+// window origins of a batched call (one per blockIdx.y)
+struct SynthOrigins {
+  long long i0[TDX_SYNTH_MAX_IMAGES], j0[TDX_SYNTH_MAX_IMAGES];
+};
+
+// one thread per cell (r, c) of the [5, h, w] window blockIdx.y at x = arange(j0, j0 + w)[c], y = arange(i0, i0 + h)[r]
 __global__ void __launch_bounds__(kThreads) synth_kernel(SynthParams p, SynthImports imp, const double* __restrict__ tables,
-                                                         int n_knots, long long i0, long long j0, int h, int w,
+                                                         int n_knots, SynthOrigins org, int h, int w,
                                                          const float* __restrict__ input, int mode,
                                                          float* __restrict__ out) {
   extern __shared__ double tab[];                 // [5][2][n_knots], then the 256 gradients
@@ -222,6 +227,8 @@ __global__ void __launch_bounds__(kThreads) synth_kernel(SynthParams p, SynthImp
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int r = (int)(i / w), c = (int)(i % w);
+  const long long i0 = org.i0[blockIdx.y], j0 = org.j0[blockIdx.y];
+  out += (size_t)blockIdx.y * kFields * n;
   float v[kFields];
   if (raw_input) {
 #pragma unroll
@@ -291,10 +298,12 @@ extern "C" int tdx_fbm_perlin(int32_t n_planes, const int32_t* seeds, const floa
   return TDX_OK;
 }
 
-extern "C" int tdx_synthetic_map(const double* tables, int32_t n_knots, const int32_t* seeds, const float* frequency,
-                                 const float* scalars, int64_t i0, int64_t j0, int32_t h, int32_t w, const float* input,
-                                 int32_t mode, const float* const* imp_values, const int64_t* imp_boxes,
-                                 const float* imp_defaults, uint32_t imp_has_default, float* out, void* stream) {
+// the checks and the launch of tdx_synthetic_map / tdx_synthetic_maps; origins: n_img (i0, j0) pairs on the host
+static int synthetic_map_launch(const double* tables, int32_t n_knots, const int32_t* seeds, const float* frequency,
+                                const float* scalars, int32_t n_img, const int64_t* origins, int32_t h, int32_t w,
+                                const float* input, int32_t mode, const float* const* imp_values,
+                                const int64_t* imp_boxes, const float* imp_defaults, uint32_t imp_has_default,
+                                float* out, void* stream) {
   TDX_REQUIRE(out, "synthetic_map: null output");
   TDX_REQUIRE((mode & ~(TDX_SYNTH_FINALIZE | TDX_SYNTH_SQRT0 | TDX_SYNTH_IMPORT | TDX_SYNTH_RAW_INPUT)) == 0,
               "synthetic_map: unknown mode bits 0x%x", (unsigned)mode);
@@ -309,8 +318,14 @@ extern "C" int tdx_synthetic_map(const double* tables, int32_t n_knots, const in
   TDX_REQUIRE((imp_has_default & ~0x1Fu) == 0, "synthetic_map: default bits 0x%x, 5 channels", (unsigned)imp_has_default);
   int rc = check_window(h, w, "synthetic_map");
   if (rc != TDX_OK) return rc;
-  TDX_REQUIRE(i0 > -(1LL << 62) && i0 < (1LL << 62) && j0 > -(1LL << 62) && j0 < (1LL << 62),
-              "synthetic_map: window origin out of range");
+  SynthOrigins org{};
+  for (int k = 0; k < n_img; ++k) {
+    const int64_t i0 = origins[2 * k], j0 = origins[2 * k + 1];
+    TDX_REQUIRE(i0 > -(1LL << 62) && i0 < (1LL << 62) && j0 > -(1LL << 62) && j0 < (1LL << 62),
+                "synthetic_map: window origin out of range");
+    org.i0[k] = (long long)i0;
+    org.j0[k] = (long long)j0;
+  }
   SynthParams p{};
   for (int f = 0; f < kFields && !input; ++f) {
     p.seed[f] = seeds[f];
@@ -339,8 +354,29 @@ extern "C" int tdx_synthetic_map(const double* tables, int32_t n_knots, const in
     imp.has_default = imp_has_default;
   }
   const size_t smem = (raw_input ? 0 : 2 * kFields * (size_t)n_knots * sizeof(double)) + 256 * sizeof(float);
-  TDX_CHECK_CUDA(launch(synth_kernel, (unsigned)(((long)h * w + kThreads - 1) / kThreads), kThreads, smem, stream, p,
-                        imp, tables, raw_input ? 0 : (int)n_knots, (long long)i0, (long long)j0, (int)h, (int)w, input,
+  TDX_CHECK_CUDA(launch(synth_kernel, dim3((unsigned)(((long)h * w + kThreads - 1) / kThreads), (unsigned)n_img),
+                        kThreads, smem, stream, p, imp, tables, raw_input ? 0 : (int)n_knots, org, (int)h, (int)w, input,
                         (int)mode, out));
   return TDX_OK;
+}
+
+extern "C" int tdx_synthetic_map(const double* tables, int32_t n_knots, const int32_t* seeds, const float* frequency,
+                                 const float* scalars, int64_t i0, int64_t j0, int32_t h, int32_t w, const float* input,
+                                 int32_t mode, const float* const* imp_values, const int64_t* imp_boxes,
+                                 const float* imp_defaults, uint32_t imp_has_default, float* out, void* stream) {
+  const int64_t origin[2] = {i0, j0};
+  return synthetic_map_launch(tables, n_knots, seeds, frequency, scalars, 1, origin, h, w, input, mode, imp_values,
+                              imp_boxes, imp_defaults, imp_has_default, out, stream);
+}
+
+extern "C" int tdx_synthetic_maps(const double* tables, int32_t n_knots, const int32_t* seeds, const float* frequency,
+                                  const float* scalars, int32_t n_img, const int64_t* origins, int32_t h, int32_t w,
+                                  int32_t mode, const float* const* imp_values, const int64_t* imp_boxes,
+                                  const float* imp_defaults, uint32_t imp_has_default, float* out, void* stream) {
+  TDX_REQUIRE(n_img >= 1 && n_img <= TDX_SYNTH_MAX_IMAGES, "synthetic_maps: %d windows, 1..%d allowed", (int)n_img,
+              TDX_SYNTH_MAX_IMAGES);
+  TDX_REQUIRE(origins, "synthetic_maps: null origins");
+  TDX_REQUIRE(!(mode & TDX_SYNTH_RAW_INPUT), "synthetic_maps: TDX_SYNTH_RAW_INPUT is not batched");
+  return synthetic_map_launch(tables, n_knots, seeds, frequency, scalars, n_img, origins, h, w, nullptr, mode,
+                              imp_values, imp_boxes, imp_defaults, imp_has_default, out, stream);
 }

@@ -26,6 +26,11 @@ device, channel 0 by `elev_coarse_pool_mode` and channel 1 by `p5_coarse_pool_mo
 averages), channels 2-5 by average, so the coarse canvas has p times fewer cells per axis (windows of (64/p)^2 at a
 stride of 48/p) and the latent stage and the climate read-out see coarser terrain.  The windows' conditioning cells and
 noise do not change.  Any other value raises ValueError in the constructor (the reference asserts only in `bind()`).
+
+`coarse_batch_size = b` (1, 2, 4, 8 or 16, keyword-only; default 1) solves up to b missing coarse windows per call
+(`stages.coarse_stage_tiles`).  Every window is bit-identical to its one-window solve, so the canvas, and everything
+read from it, does not depend on b.  It is a serving choice, like `latents_batch_size`, and is not written to
+config.json.  Any other value raises ValueError in the constructor.
 """
 from __future__ import annotations
 
@@ -39,7 +44,8 @@ import torch
 
 from ..scheduler import EDMDPMSolverMultistepScheduler
 from .lazy_canvas import LazyCanvas, TensorWindow
-from .stages import coarse_geometry, coarse_stage_tile, decoder_stage_tile, latent_stage_tiles
+from .stages import (COARSE_BATCH_SIZES, coarse_geometry, coarse_stage_tile, coarse_stage_tiles, decoder_stage_tile,
+                     latent_stage_tiles)
 from .tiling import linear_weight_window
 
 # seed offsets of the latent stage's noise fields: _build_latent_stage (world_pipeline.py:1133-1203) passes 5819 to the
@@ -71,8 +77,8 @@ class WorldPipeline:
     BASE_MODEL_FOLDER = "base_model"
     DECODER_MODEL_FOLDER = "decoder_model"
     config_name = "config.json"
-    ignore_for_config = ["seed", "latents_batch_size", "log_mode", "cache_limit", "caching_strategy", "torch_compile",
-                         "dtype"]
+    ignore_for_config = ["seed", "latents_batch_size", "coarse_batch_size", "log_mode", "cache_limit",
+                         "caching_strategy", "torch_compile", "dtype"]
 
     def __init__(self, seed: int | None = None, latents_batch_size=(1, 2, 4, 8, 16), native_resolution: float = 90.0, *,
                  T: int = 2, log_mode: str = "info", torch_compile: bool = False, dtype: str | None = None,
@@ -82,7 +88,7 @@ class WorldPipeline:
                  coarse_means: list | None = None, coarse_stds: list | None = None, caching_strategy: str = "direct",
                  cache_limit: int | None = 100 * 1024 * 1024, onestep_latent: bool = False,
                  decoder_tile_size: int = 512, decoder_tile_stride: int = 384, conditioning_fn=None,
-                 synthetic_map_stats=None, **deprecated_kwargs):
+                 synthetic_map_stats=None, coarse_batch_size: int = 1, **deprecated_kwargs):
         from .noise import next_seed
         if T not in (1, 2):
             raise ValueError(f"T must be 1 or 2, got {T}")
@@ -90,6 +96,12 @@ class WorldPipeline:
             raise ValueError("pass either conditioning_fn or synthetic_map_stats, not both")
         coarse_geometry(coarse_pooling)                  # ValueError unless it divides 64 and 48 (world_pipeline.py:969-970)
         coarse_pooling = operator.index(coarse_pooling)
+        try:
+            self.coarse_batch_size = operator.index(coarse_batch_size)
+        except TypeError:
+            self.coarse_batch_size = None
+        if self.coarse_batch_size not in COARSE_BATCH_SIZES:
+            raise ValueError(f"coarse_batch_size must be one of {list(COARSE_BATCH_SIZES)}; got {coarse_batch_size!r}")
         self.T = T
         self.seed = (int(seed) & 0xFFFFFFFFFFFFFFFF) if seed is not None else next_seed(None)
         sizes = [latents_batch_size] if isinstance(latents_batch_size, int) else sorted(latents_batch_size)
@@ -230,6 +242,9 @@ class WorldPipeline:
             get_diffusion_solve(self.coarse_model, EDMDPMSolverMultistepScheduler(sigma_min=0.002, sigma_max=80,
                                                                                    sigma_data=0.5), 1, 64, 64,
                                 20).prog.instantiate()
+            for m in (m for m in COARSE_BATCH_SIZES if 1 < self.coarse_batch_size and m <= self.coarse_batch_size):
+                get_diffusion_solve(self.coarse_model, EDMDPMSolverMultistepScheduler(
+                    sigma_min=0.002, sigma_max=80, sigma_data=0.5), m, 64, 64, 20, batch_invariant=True).prog.instantiate()
 
     # ------------------------------------------------------------------ conditioning (injected; see module docstring)
     def _set_cond(self, cond_snr) -> None:
@@ -336,8 +351,23 @@ class WorldPipeline:
                                      self.kwargs["coarse_stds"], 20, pool, self.kwargs["elev_coarse_pool_mode"],
                                      self.kwargs["p5_coarse_pool_mode"])
 
-        coarse = self._canvas("coarse", 7, f_coarse, TensorWindow((7, c_tile, c_tile), (7, c_stride, c_stride)), dev,
-                              cache_limit=lim)
+        def f_coarse_batch(ctxs):
+            origins = [(i * 48, j * 48) for _, i, j in ctxs]
+            if self._synthetic is not None:
+                smaps = self._synthetic.conditioning_windows(origins, 64, self._device_imports(), device=self.device)
+            else:
+                smaps = [self._conditioning_model_input(a, a + 64, b, b + 64) for a, b in origins]
+            return coarse_stage_tiles(self.coarse_model, coarse_sched, self.seed, ctxs, smaps, self._t_cond,
+                                      self._cond_inputs, ww_coarse, self.kwargs["coarse_means"],
+                                      self.kwargs["coarse_stds"], 20, pool, self.kwargs["elev_coarse_pool_mode"],
+                                      self.kwargs["p5_coarse_pool_mode"])
+
+        # coarse_batch_size > 1: missing windows are solved up to that many at a time, each bit-identical to its
+        # one-window solve (stages.coarse_stage_tiles), so the canvas does not depend on the batching
+        batched = self.coarse_batch_size > 1
+        coarse = self._canvas("coarse", 7, f_coarse_batch if batched else f_coarse,
+                              TensorWindow((7, c_tile, c_tile), (7, c_stride, c_stride)), dev,
+                              batch_size=self.coarse_batch_size if batched else None, cache_limit=lim)
 
         # ---- latents: 64^2 tiles, stride 32; T=2: two consistency phases with a blend in between, T=1: both phases per
         # tile; batches padded to the legal sizes so that only a handful of plans exist
@@ -645,7 +675,7 @@ class TerrainPipeline(WorldPipeline):
                  t_inter: float | None = None, residual_mean: float | None = None, residual_std: float | None = None,
                  native_resolution: float = 90.0, cache_limit: int | None = None, coarse_pooling: int = 1,
                  elev_coarse_pool_mode: str = "avg", p5_coarse_pool_mode: str = "avg", synthetic_map_stats=None,
-                 frequency_mult: list | None = None):
+                 frequency_mult: list | None = None, coarse_batch_size: int = 1):
         super().__init__(seed=seed, latents_batch_size=latents_batch_size, native_resolution=native_resolution,
                          latent_compression=latent_compression, cond_snr=[float(v) for v in cond_snr],
                          coarse_pooling=coarse_pooling, elev_coarse_pool_mode=elev_coarse_pool_mode,
@@ -656,7 +686,8 @@ class TerrainPipeline(WorldPipeline):
                          synthetic_map_stats=synthetic_map_stats, frequency_mult=frequency_mult,
                          histogram_raw=[float(v) for v in torch.as_tensor(histogram_raw).flatten()],
                          cond_input_mean=[float(v) for v in torch.as_tensor(latents_means).flatten()],
-                         cond_input_std=[float(v) for v in torch.as_tensor(latents_stds).flatten()], t_inter=t_inter)
+                         cond_input_std=[float(v) for v in torch.as_tensor(latents_stds).flatten()], t_inter=t_inter,
+                         coarse_batch_size=coarse_batch_size)
         self.coarse_model, self.base_model, self.decoder_model = coarse_model, base_model, decoder_model
         self._host_views = False
         self._build_hierarchy()

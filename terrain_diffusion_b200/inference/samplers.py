@@ -46,12 +46,12 @@ def _solve_cache(model):
 
 
 def get_diffusion_solve(model, scheduler, n, h, w, num_steps, step_range=None, guide=None, guidance_scale: float = 1.0,
-                        score_scaling: float = 1.0) -> DiffusionSolve:
+                        score_scaling: float = 1.0, batch_invariant: bool = False) -> DiffusionSolve:
     """Cached fused N-step solve (or one phase of it: step_range).  The key is everything the solve bakes in: the
     sigma table and the per-step order schedule (they cover sigma_min/max/rho/schedule, scaling_p/scaling_t,
     lower_order_final, euler_at_final, ...) plus the options that change the update formula, and for a guided solve
     the guide's weights, the guidance scale and the score scaling.  The caller's scheduler is put in the state the
-    reference leaves it in (`set_timesteps(num_steps)`) on a cache hit too."""
+    reference leaves it in (`set_timesteps(num_steps)`) on a cache hit too.  batch_invariant: see DiffusionSolve."""
     scheduler.set_timesteps(num_steps)
     c = scheduler.config
     key = (n, h, w, num_steps, None if step_range is None else tuple(int(v) for v in step_range),
@@ -63,11 +63,13 @@ def get_diffusion_solve(model, scheduler, n, h, w, num_steps, step_range=None, g
         key += ("guide", id(guide.folded()), float(guidance_scale))
     if score_scaling != 1.0:
         key += ("score_scaling", float(score_scaling))
+    if batch_invariant:
+        key += ("batch_invariant",)
     cache = _solve_cache(model)
     if key not in cache:
         cache[key] = DiffusionSolve(model, scheduler, n, h, w, num_steps, step_range=step_range,
                                     guide=guide if guided else None, guidance_scale=guidance_scale,
-                                    score_scaling=score_scaling)
+                                    score_scaling=score_scaling, batch_invariant=batch_invariant)
     return cache[key]
 
 

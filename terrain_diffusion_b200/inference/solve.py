@@ -50,7 +50,7 @@ class DiffusionSolve:
     exactly the unguided program (the reference skips the guide forward then too)."""
 
     def __init__(self, model, scheduler, n: int, h: int, w: int, num_steps: int, step_range=None, coef_rows=None,
-                 guide=None, guidance_scale: float = 1.0, score_scaling: float = 1.0):
+                 guide=None, guidance_scale: float = 1.0, score_scaling: float = 1.0, batch_invariant: bool = False):
         """coef_rows: explicit per-step tables [dict(c_in, t, c_skip, c_out, r, k)] instead of a scheduler's (the
         TrigFlow consistency step is the same fused program with other numbers: consistency_rows()).
         step_range = (i0, i1): only steps i0 .. i1-1 of the `num_steps` schedule (one PHASE of a multi-phase
@@ -58,7 +58,10 @@ class DiffusionSolve:
         from a blended canvas, so the multistep history is empty there: its first step is first order, exactly like
         a scheduler whose state was reset and positioned at step i0.
         guide / guidance_scale: two-model guidance; score_scaling: the EDM score scaling alpha of the reference's
-        decoder sampler, folded into the coefficient rows (fold_score_scaling)."""
+        decoder sampler, folded into the coefficient rows (fold_score_scaling).
+        batch_invariant: each of the n tiles comes out bit-identical to a one-tile solve of it: the launches use their
+        one-image item shapes (UNetEmitter), and the host embedding is computed for one tile and shared, so every
+        conditional input of run() must then be a single row."""
         fw = model.folded()
         dev = fw.device
         self.guided = guide is not None and float(guidance_scale) != 1.0
@@ -83,6 +86,7 @@ class DiffusionSolve:
                       for c, i in zip(co, range(i0, i1))]
             num_steps = i1 - i0                  # from here on: the number of steps this solve runs
         self.model, self.n, self.h, self.w, self.num_steps = model, n, h, w, num_steps
+        self.batch_invariant = batch_invariant
         cs = fw.out_channels
         cc = fw.in_channels - cs
         if self.guided:
@@ -104,11 +108,12 @@ class DiffusionSolve:
         self.x0_prev = torch.zeros_like(self.sample)
         self.prog = UNetProgram(fw.device)
         # the noise labels of all steps are known up front: ONE embed launch produces every step's modulation vectors
-        em = UNetEmitter(fw, n, h, w, cvec_sets=num_steps)
+        em = UNetEmitter(fw, n, h, w, cvec_sets=num_steps, batch_invariant=batch_invariant)
         self.host_emb = len(model.conditional_layers) > 0 or not fw.pos_emb
         if self.guided:
             check_plannable(gfw, "guide model")
-            gem = UNetEmitter(gfw, n, h, w, cvec_sets=num_steps)          # its own arena and modulation vectors
+            gem = UNetEmitter(gfw, n, h, w, cvec_sets=num_steps,          # its own arena and modulation vectors
+                              batch_invariant=batch_invariant)
             self.guide_out = torch.zeros_like(self.sample)
         if self.host_emb:
             # conditional models (coarse: five float conditions): the 256-wide embeddings of all steps are computed
@@ -144,17 +149,28 @@ class DiffusionSolve:
         solver's state buffer -- copy it before the next run)."""
         if self.host_emb:
             # conditional models: ONE batched evaluation of compute_embeddings for the labels of all steps
+            labels = self.labels[:, :1].reshape(-1) if self.batch_invariant else self.labels.reshape(-1)
+            if self.batch_invariant and any(c.shape[0] != 1 for c in (conditional_inputs or [])):
+                raise ValueError("a batch-invariant solve shares its conditional inputs: pass one row each")
             ci = [c.to(self.labels.device).repeat(self.num_steps, *([1] * (c.dim() - 1)))
                   for c in (conditional_inputs or [])]
-            self.emb_all.copy_(self.model._host_embedding(self.labels.reshape(-1), ci))
+            self._set_embedding(self.emb_all, self.model._host_embedding(labels, ci))
             if self.guided:
-                self.guide_emb_all.copy_(self.guide._host_embedding(self.labels.reshape(-1), ci))
+                self._set_embedding(self.guide_emb_all, self.guide._host_embedding(labels, ci))
         self.sample.copy_(noise)
         if cond is not None:
             self.cond.copy_(cond)
         self.x0_prev.zero_()
         self.prog.run(use_graph)
         return self.sample
+
+    def _set_embedding(self, dst: torch.Tensor, emb: torch.Tensor) -> None:
+        """dst [num_steps * n, E] (step-major) <- emb: the same rows, or with batch_invariant one row per step that
+        every tile shares (the host GEMMs then see the one-tile shape, whatever n is)."""
+        if self.batch_invariant:
+            dst.view(self.num_steps, self.n, -1).copy_(emb.view(self.num_steps, 1, -1).expand(-1, self.n, -1))
+        else:
+            dst.copy_(emb)
 
 
 def consistency_rows(t: float, sigma_data: float = 0.5, from_unit_noise: bool = False, out_scale: float = 1.0):

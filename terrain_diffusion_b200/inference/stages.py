@@ -13,7 +13,9 @@ around the U-Net, `.item()`, D2H -- is organised here around ONE fused program p
                        (tdx_window_to_cond).
   coarse stage         `get_diffusion_solve`: the 20-step DPM-Solver++ solve as one graph, the embeddings of all steps
                        from one batched call.  De-normalisation, the channel-1 difference, `coarse_pooling` and the
-                       packed output are one launch (tdx_coarse_epilogue).
+                       packed output are one launch (tdx_coarse_epilogue).  `coarse_stage_tiles` solves a batch of
+                       windows: its inputs are one launch (tdx_coarse_condition) and its solve is batch-invariant, so
+                       every window is bit-identical to its `coarse_stage_tile`.
 
 Noise comes from the bit-compatible GPU generator (same seeds as the reference), nothing synchronises with the host and
 nothing leaves the GPU.  Taken as arguments: the synthetic conditioning map of the coarse stage (built on the device by
@@ -260,3 +262,74 @@ def coarse_stage_tile(model, scheduler, seed: int, ctx, synthetic_map: torch.Ten
                        conditional_inputs=[_const_on(dev, c) for c in cond_inputs])
     return coarse_epilogue(sample.contiguous(), means, stds, _f32(weight_window, dev), pool_size, elev_pool_mode,
                            p5_pool_mode, float(scheduler.config.sigma_data))[0]
+
+
+def coarse_condition(maps: torch.Tensor, cond_noise: torch.Tensor, sample_noise: torch.Tensor, means: torch.Tensor,
+                     stds: torch.Tensor, t_cond: torch.Tensor, sigma0: float) -> tuple:
+    """The solve inputs of n coarse windows in one launch (world_pipeline.py:921-933), bit for bit with
+    coarse_stage_tile's torch ops: cond = cos(t) * ((map - mean) / std) + sin(t) * cond_noise over the five map channels
+    and sample = sample_noise * sigma0.  maps, cond_noise [n, 5, 64, 64] and sample_noise [n, 6, 64, 64] fp32 on one
+    device; means / stds: the 6 model statistics (the map's channels use 0, 2, 3, 4, 5); t_cond: the 5 noise angles.
+    Returns (cond, sample)."""
+    n = maps.shape[0]
+    dev = maps.device
+    shapes = ((maps, (n, 5, COARSE_TILE, COARSE_TILE)), (cond_noise, (n, 5, COARSE_TILE, COARSE_TILE)),
+              (sample_noise, (n, 6, COARSE_TILE, COARSE_TILE)))
+    for t, shape in shapes:
+        if tuple(t.shape) != shape or t.dtype != torch.float32 or not t.is_contiguous() or t.device != dev:
+            raise ValueError(f"coarse_condition: expected a contiguous fp32 {list(shape)} tensor on {dev}, got "
+                             f"{t.dtype} {tuple(t.shape)} on {t.device}")
+    sel = [0, 2, 3, 4, 5]                                        # model statistics of the map's five channels (:925)
+    m5, s5 = means[sel].contiguous(), stds[sel].contiguous()
+    tc = _const_on(dev, t_cond).view(-1)
+    cos_t, sin_t = torch.cos(tc), torch.sin(tc)                  # the same device ops as coarse_stage_tile's
+    cond = torch.empty_like(maps)
+    sample = torch.empty_like(sample_noise)
+    L.call(L.lib().tdx_coarse_condition, dev, cond.data_ptr(), sample.data_ptr(), maps.data_ptr(),
+           cond_noise.data_ptr(), sample_noise.data_ptr(), m5.data_ptr(), s5.data_ptr(), cos_t.data_ptr(),
+           sin_t.data_ptr(), float(sigma0), n, COARSE_TILE * COARSE_TILE)
+    return cond, sample
+
+
+COARSE_BATCH_SIZES = (1, 2, 4, 8, 16)
+
+
+@torch.no_grad()
+def coarse_stage_tiles(model, scheduler, seed: int, ctxs, synthetic_maps, t_cond: torch.Tensor, cond_inputs,
+                       weight_window: torch.Tensor, coarse_means, coarse_stds, num_steps: int = 20, pool_size: int = 1,
+                       elev_pool_mode: str = "avg", p5_pool_mode: str = "avg") -> list:
+    """coarse_stage_tile for a batch of windows: ctxs [(0, i, j), ...] with their raw [5, 64, 64] conditioning maps
+    (a list of CUDA or CPU tensors, or one [n, 5, 64, 64] tensor).  Returns the packed [7, 64/p, 64/p] tiles (views of
+    one device tensor), each bit-identical to coarse_stage_tile of its window whatever the rest of the batch is.  The
+    batch is padded to the next of COARSE_BATCH_SIZES, so that at
+    most five solve programs exist per model.  At most 16 windows per call."""
+    coarse_geometry(pool_size)                                   # argument errors before any device work
+    if len(ctxs) != len(synthetic_maps):
+        raise ValueError(f"coarse_stage_tiles: {len(ctxs)} windows but {len(synthetic_maps)} conditioning maps")
+    if not ctxs:
+        return []
+    top = COARSE_BATCH_SIZES[-1]
+    if len(ctxs) > top:
+        raise ValueError(f"coarse_stage_tiles: {len(ctxs)} windows, at most {top} per call")
+    dev = model.device
+    n, T = len(ctxs), COARSE_TILE
+    means = _const_on(dev, torch.as_tensor(coarse_means, dtype=torch.float32))
+    stds = _const_on(dev, torch.as_tensor(coarse_stds, dtype=torch.float32))
+    if isinstance(synthetic_maps, torch.Tensor):
+        maps = _f32(synthetic_maps, dev)
+    elif all(torch.as_tensor(m).device.type == "cpu" for m in synthetic_maps):   # host maps: ONE copy
+        maps = _f32(torch.stack([torch.as_tensor(m) for m in synthetic_maps]), dev)
+    else:
+        maps = torch.stack([_f32(torch.as_tensor(m), dev) for m in synthetic_maps])
+    origins = [(c[1] * COARSE_STRIDE, c[2] * COARSE_STRIDE) for c in ctxs]
+    cond_noise = gaussian_noise_patches(seed, origins, T, T, 5, T, T, device=dev)
+    sample_noise = gaussian_noise_patches(seed + 1, origins, T, T, 6, T, T, device=dev)
+    m = padded_batch_size(n, top)
+    solve = get_diffusion_solve(model, scheduler, m, T, T, num_steps, batch_invariant=True)
+    cond, sample = coarse_condition(maps, cond_noise, sample_noise, means, stds, t_cond, float(scheduler.sigmas[0]))
+    if m > n:      # padding repeats window 0; a batch-invariant solve keeps the real windows' bits
+        cond = torch.cat([cond, cond[:1].expand(m - n, -1, -1, -1)], dim=0)
+        sample = torch.cat([sample, sample[:1].expand(m - n, -1, -1, -1)], dim=0)
+    out = solve.run(sample, cond, conditional_inputs=[_const_on(dev, c) for c in cond_inputs])
+    return list(coarse_epilogue(out[:n].contiguous(), means, stds, _f32(weight_window, dev), pool_size, elev_pool_mode,
+                                p5_pool_mode, float(scheduler.config.sigma_data)))

@@ -32,6 +32,7 @@ STATS_CACHE_PATH = "data/global/synthetic_map_stats.json"     # synthetic_map.py
 MAX_PLANES = 8                                                 # TDX_FBM_MAX_PLANES
 MAX_KNOTS = 512                                                # TDX_SYNTH_MAX_KNOTS
 FINALIZE, SQRT0, IMPORT, RAW_INPUT = 1, 2, 4, 8                # TDX_SYNTH_* mode bits
+MAX_WINDOWS = 16                                                # TDX_SYNTH_MAX_IMAGES: windows per tdx_synthetic_maps
 SCALAR_KEYS = ("a_temp_std", "b_temp_std", "temp_std_p1", "temp_std_p99")
 
 
@@ -247,6 +248,25 @@ class SyntheticMap:
         if imports is None:
             return self(cj0, ci0, cj1, ci1, device=device)
         return self._launch(ci0, cj0, ci1 - ci0, cj1 - cj0, IMPORT | SQRT0, device, imports=imports[:4])
+
+    def conditioning_windows(self, origins, size: int, imports=None, device=None) -> torch.Tensor:
+        """fp32 [n, 5, size, size]: `conditioning(ci0, ci0 + size, cj0, cj0 + size, imports)` for every (ci0, cj0) of
+        `origins`, in one launch per 16 windows, each bit-identical to its own call."""
+        dev = _device(device if device is not None else self.device)
+        size = _int("size", size)
+        org = np.array([(_int("ci0", a), _int("cj0", b)) for a, b in origins], np.int64).reshape(-1, 2)
+        if size < 1 or len(org) == 0:
+            raise ValueError(f"conditioning_windows needs windows and a positive size, got {len(org)} of {size}")
+        out = torch.empty((len(org), 5, size, size), dtype=torch.float32, device=dev)
+        mode = IMPORT | SQRT0 if imports is not None else FINALIZE | SQRT0
+        ptrs, boxes, defaults, has_default = imports[:4] if imports is not None else (None, None, None, 0)
+        tables = self.tables(dev)
+        for g in range(0, len(org), MAX_WINDOWS):
+            chunk = np.ascontiguousarray(org[g:g + MAX_WINDOWS])
+            L.call(L.lib().tdx_synthetic_maps, dev, tables.data_ptr(), self.n_knots, self._seeds.ctypes.data,
+                   self._freq.ctypes.data, self._scalars.ctypes.data, len(chunk), chunk.ctypes.data, size, size, mode,
+                   ptrs, boxes, defaults, has_default, out[g].data_ptr())
+        return out
 
 
 def device_imports(imports: dict, origins: dict, defaults: dict, device) -> tuple:

@@ -318,10 +318,13 @@ class UNetProgram:
 class UNetEmitter:
     """Allocates the activation arena for (n, h, w) and appends the launches of one U-Net evaluation to a program."""
 
-    def __init__(self, fw: FoldedWeights, n: int, h: int, w: int, cvec_sets: int = 1):
+    def __init__(self, fw: FoldedWeights, n: int, h: int, w: int, cvec_sets: int = 1, batch_invariant: bool = False):
         """cvec_sets: how many independent label sets (e.g. solver steps) share this arena; the modulation vectors of
-        all of them are produced by ONE embed launch (emit_embed) and selected per evaluation with `cvec_set`."""
+        all of them are produced by ONE embed launch (emit_embed) and selected per evaluation with `cvec_set`.
+        batch_invariant: every implicit-GEMM launch uses the item shape (N, split-K) its one-image plan would, the
+        other images as extra M tiles, so each image's result is bit-identical to a one-image program's."""
         self.cvec_sets = cvec_sets
+        self.batch_invariant = batch_invariant
         downs = sum(b.get("resample") == "down" for b in fw.enc)
         ups = sum(b.get("resample") == "up" for b in fw.dec)
         need = 8 * 2 ** downs
@@ -410,12 +413,19 @@ class UNetEmitter:
             d.a_channels[i] = ch
             d.a_taps[i] = taps
         d.n_seg = len(segs)
-        n_item = L.igemm_choose_n(cout, self.n, h, w, [(ch, taps) for _, ch, taps in segs])
+        n_item = L.igemm_choose_n(cout, 1 if self.batch_invariant else self.n, h, w, [(ch, taps) for _, ch, taps in segs])
         d.n_per_item = n_item
         d.b_packed = self.fw.packed(wkey, n_item).data_ptr()
         d.c_out = cout
         d.n_img, d.height, d.width = self.n, h, w
         return d
+
+    def _add_igemm(self, prog, d):
+        if self.batch_invariant:
+            one = L.TdxIgemmDesc.from_buffer_copy(d)
+            one.n_img, one.ksplit = 1, 0
+            d.ksplit = L.igemm_launch_shape(one)[1]
+        prog.add("igemm", d)
 
     def _finish_block(self, prog, d, b, key, cout, h, w, nxt, enc_index):
         """Tail of UNetBlock.forward after conv_res1 (`d` = its launch, residual already configured):
@@ -424,19 +434,19 @@ class UNetEmitter:
         if not b["heads"]:
             d.clip = fw.clip
             cur = self._emit_outputs(d, key, cout, h, w, nxt, enc_index)
-            prog.add("igemm", d)
+            self._add_igemm(prog, d)
             return cur
         # ---- attention: x1 = mp_sum(x, y) un-clipped -> q, k, v (1x1) -> softmax core -> proj (1x1) + mp_sum + clip
         x1 = self.act(key + "x1", cout, h, w)
         d.clip = 0.0
         self._set_out(d, 0, x1, L.OUT_RAW)
-        prog.add("igemm", d)
+        self._add_igemm(prog, d)
         qkv = []
         for nm in ("q", "k", "v"):
             t = self.act(key + nm, cout, h, w)
             dq = self._igemm(prog, [(x1, cout, 1)], key + nm, cout, h, w)
             self._set_out(dq, 0, t, L.OUT_RAW)
-            prog.add("igemm", dq)
+            self._add_igemm(prog, dq)
             qkv.append(t)
         yat = self.act(key + "attn_y", cout, h, w)
         ad = L.TdxAttnDesc()
@@ -451,7 +461,7 @@ class UNetEmitter:
         dp.resid_scale = (1 - ta) / math.sqrt((1 - ta) ** 2 + ta ** 2)
         dp.clip = fw.clip
         cur = self._emit_outputs(dp, key, cout, h, w, nxt, enc_index)
-        prog.add("igemm", dp)
+        self._add_igemm(prog, dp)
         return cur
 
     # ------------------------------------------------------------------ embedding / modulation vectors
@@ -538,7 +548,7 @@ class UNetEmitter:
                 prog.add("im2col", im)
                 d = self._igemm(prog, [(cols, kpad, 1)], "conv_in.im2col", cout, h, w)
                 cur = self._emit_outputs(d, key, cout, h, w, nxt, enc_index)
-                prog.add("igemm", d)
+                self._add_igemm(prog, d)
             elif b["mode"] == "enc":
                 resid_sp = L.SP_SAME
                 if b["resample"] == "down":
@@ -551,7 +561,7 @@ class UNetEmitter:
                     a_in = self.act(key + "a0", cout, h, w)
                     self._set_out(d, 0, xn, L.OUT_RAW)
                     self._set_out(d, 1, a_in, L.OUT_SILU, L.SP_SAME, 1.0)
-                    prog.add("igemm", d)
+                    self._add_igemm(prog, d)
                     resid, resid_pn, resid_inv = xn, 0, None
                 else:
                     a_in, resid, resid_pn = cur["act"], cur["raw"], 1
@@ -563,7 +573,7 @@ class UNetEmitter:
                 d.epi_flags = L.EPI_EMB_SILU
                 d.cvec = self._cvec_ptr(key, cout, cvec_set)
                 self._set_out(d, 0, hbuf, L.OUT_RAW)
-                prog.add("igemm", d)
+                self._add_igemm(prog, d)
                 d = self._igemm(prog, [(hbuf, cout, 9)], key + "res1", cout, h, w)
                 d.epi_flags = L.EPI_RESID
                 d.resid = resid.data_ptr()
@@ -590,7 +600,7 @@ class UNetEmitter:
                 d.epi_flags = L.EPI_EMB_SILU
                 d.cvec = self._cvec_ptr(key, cout, cvec_set)
                 self._set_out(d, 0, hbuf, L.OUT_RAW)
-                prog.add("igemm", d)
+                self._add_igemm(prog, d)
                 if b.get("concat"):
                     d = self._igemm(prog, [(hbuf, cout, 9), (cur["raw"], cx, 1), (sk["raw"], cs, 1)], key + "res1",
                                     cout, h, w)
