@@ -78,7 +78,8 @@ typedef struct TdxIgemmDesc {
   int32_t resid_spatial;   /* TDX_SP_SAME | TDX_SP_UP2 (r is H/2 x W/2) | TDX_SP_DOWN2 (r is 2H x 2W)            */
   int32_t resid_pnorm;     /* r' = pixelnorm(r) over channels (unet_block.py:121) when non-zero                  */
   float resid_scale;
-  float clip;              /* > 0: v = clamp(v, -clip, +clip) after the residual (unet_block.py:153-154); 0: off  */
+  float clip;              /* > 0: v = clamp(v, -clip, +clip) after the residual (unet_block.py:153-154), NaN stays
+                            * NaN as in torch.clip; 0: off                                                          */
   TdxOutSpec out[3];
   /* Pixel-norm side channel (fp32 [n_img][H][W] planes).  A launch that computes the pixel-norm of its result (a
    * TDX_OUT_PNORM_SILU output or TDX_EPI_PNORM) can also store the per-pixel factor 1 / (1e-4 + rms over c_out) in

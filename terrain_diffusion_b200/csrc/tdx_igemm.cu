@@ -784,7 +784,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CU
           }
           if (p.clip > 0.f) {
 #pragma unroll
-            for (int i = 0; i < kChunk; ++i) v[i] = fminf(fmaxf(v[i], -p.clip), p.clip);
+            for (int i = 0; i < kChunk; ++i) v[i] = clamp_keep_nan(v[i], p.clip);
           }
         };
         auto emit_v = [&](int ck, float (&v)[kChunk], float inv) {

@@ -208,6 +208,14 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_
 }
 
 // ---------------------------------------------------------------- math
+// torch.clamp(x, -c, c) for c > 0: NaN stays NaN (fminf / fmaxf would return the bound).  max.NaN / min.NaN (sm_80+)
+// return NaN when either operand is NaN and are fmaxf / fminf otherwise, so finite and infinite results are unchanged.
+__device__ __forceinline__ float clamp_keep_nan(float x, float c) {
+  float y;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(y) : "f"(x), "f"(-c));
+  asm("min.NaN.f32 %0, %0, %1;" : "+f"(y) : "f"(c));
+  return y;
+}
 __device__ __forceinline__ float tanh_approx(float x) {
   float y;
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
