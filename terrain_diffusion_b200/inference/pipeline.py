@@ -31,6 +31,10 @@ noise do not change.  Any other value raises ValueError in the constructor (the 
 (`stages.coarse_stage_tiles`).  Every window is bit-identical to its one-window solve, so the canvas, and everything
 read from it, does not depend on b.  It is a serving choice, like `latents_batch_size`, and is not written to
 config.json.  Any other value raises ValueError in the constructor.
+
+`decoder_batch_size = b` (one of stages.DECODER_BATCH_SIZES, keyword-only; default 1) does the same for the decoder
+stage: up to b missing residual windows per call (`stages.decoder_stage_tiles`), each bit-identical to its one-window
+solve.  Its consistency program holds b windows of activations (DESIGN.md section 5 gives the measured memory).
 """
 from __future__ import annotations
 
@@ -44,8 +48,8 @@ import torch
 
 from ..scheduler import EDMDPMSolverMultistepScheduler
 from .lazy_canvas import LazyCanvas, TensorWindow
-from .stages import (COARSE_BATCH_SIZES, coarse_geometry, coarse_stage_tile, coarse_stage_tiles, decoder_stage_tile,
-                     latent_stage_tiles)
+from .stages import (COARSE_BATCH_SIZES, DECODER_BATCH_SIZES, coarse_geometry, coarse_stage_tile, coarse_stage_tiles,
+                     decoder_stage_tile, decoder_stage_tiles, latent_stage_tiles)
 from .tiling import linear_weight_window
 
 # seed offsets of the latent stage's noise fields: _build_latent_stage (world_pipeline.py:1133-1203) passes 5819 to the
@@ -59,6 +63,17 @@ DEFAULT_COARSE_MEANS = [-37.67916460232751, 2.22578822145657, 18.030293275011356
                         1350.1259248456176, 52.444339366764396]
 DEFAULT_COARSE_STDS = [39.68515115440358, 3.0981253981231522, 8.940333096712806, 322.25238547630295,
                        856.3430083394657, 30.982620765341043]
+
+
+def _batch_size(name: str, value, legal: tuple) -> int:
+    """`value` as an int if it is one of `legal`, else ValueError (a float or a string is not a batch size)."""
+    try:
+        size = operator.index(value)
+    except TypeError:
+        size = None
+    if size not in legal:
+        raise ValueError(f"{name} must be one of {list(legal)}; got {value!r}")
+    return size
 
 
 class _HostView:
@@ -77,8 +92,8 @@ class WorldPipeline:
     BASE_MODEL_FOLDER = "base_model"
     DECODER_MODEL_FOLDER = "decoder_model"
     config_name = "config.json"
-    ignore_for_config = ["seed", "latents_batch_size", "coarse_batch_size", "log_mode", "cache_limit",
-                         "caching_strategy", "torch_compile", "dtype"]
+    ignore_for_config = ["seed", "latents_batch_size", "coarse_batch_size", "decoder_batch_size", "log_mode",
+                         "cache_limit", "caching_strategy", "torch_compile", "dtype"]
 
     def __init__(self, seed: int | None = None, latents_batch_size=(1, 2, 4, 8, 16), native_resolution: float = 90.0, *,
                  T: int = 2, log_mode: str = "info", torch_compile: bool = False, dtype: str | None = None,
@@ -88,7 +103,8 @@ class WorldPipeline:
                  coarse_means: list | None = None, coarse_stds: list | None = None, caching_strategy: str = "direct",
                  cache_limit: int | None = 100 * 1024 * 1024, onestep_latent: bool = False,
                  decoder_tile_size: int = 512, decoder_tile_stride: int = 384, conditioning_fn=None,
-                 synthetic_map_stats=None, coarse_batch_size: int = 1, **deprecated_kwargs):
+                 synthetic_map_stats=None, coarse_batch_size: int = 1, decoder_batch_size: int = 1,
+                 **deprecated_kwargs):
         from .noise import next_seed
         if T not in (1, 2):
             raise ValueError(f"T must be 1 or 2, got {T}")
@@ -96,12 +112,8 @@ class WorldPipeline:
             raise ValueError("pass either conditioning_fn or synthetic_map_stats, not both")
         coarse_geometry(coarse_pooling)                  # ValueError unless it divides 64 and 48 (world_pipeline.py:969-970)
         coarse_pooling = operator.index(coarse_pooling)
-        try:
-            self.coarse_batch_size = operator.index(coarse_batch_size)
-        except TypeError:
-            self.coarse_batch_size = None
-        if self.coarse_batch_size not in COARSE_BATCH_SIZES:
-            raise ValueError(f"coarse_batch_size must be one of {list(COARSE_BATCH_SIZES)}; got {coarse_batch_size!r}")
+        self.coarse_batch_size = _batch_size("coarse_batch_size", coarse_batch_size, COARSE_BATCH_SIZES)
+        self.decoder_batch_size = _batch_size("decoder_batch_size", decoder_batch_size, DECODER_BATCH_SIZES)
         self.T = T
         self.seed = (int(seed) & 0xFFFFFFFFFFFFFFFF) if seed is not None else next_seed(None)
         sizes = [latents_batch_size] if isinstance(latents_batch_size, int) else sorted(latents_batch_size)
@@ -238,6 +250,9 @@ class WorldPipeline:
             T_ = self.decoder_tile_size
             get_consistency_solve(self.decoder_model, 1, T_, T_, float(self.t_init), sd, from_unit_noise=True,
                                   out_scale=1.0 / sd).prog.instantiate()
+            for m in (m for m in DECODER_BATCH_SIZES if 1 < m <= self.decoder_batch_size):
+                get_consistency_solve(self.decoder_model, m, T_, T_, float(self.t_init), sd, from_unit_noise=True,
+                                      out_scale=1.0 / sd, batch_invariant=True).prog.instantiate()
         if self.coarse_model is not None:
             get_diffusion_solve(self.coarse_model, EDMDPMSolverMultistepScheduler(sigma_min=0.002, sigma_max=80,
                                                                                    sigma_data=0.5), 1, 64, 64,
@@ -403,9 +418,17 @@ class WorldPipeline:
             return decoder_stage_tile(self.decoder_model, self.seed, ctx, latents_window, ww_t, [self.t_init], T_, S_,
                                       latent_compression=lc)
 
-        residual = self._canvas("residual", 2, f_dec, TensorWindow((2, T_, T_), (2, S_, S_)), dev, args=(latents,),
+        def f_dec_batch(ctxs, latents_windows):
+            return decoder_stage_tiles(self.decoder_model, self.seed, ctxs, latents_windows, ww_t, [self.t_init], T_,
+                                       S_, latent_compression=lc)
+
+        # decoder_batch_size > 1: missing windows are solved up to that many at a time, each bit-identical to its
+        # one-window solve (stages.decoder_stage_tiles)
+        batched = self.decoder_batch_size > 1
+        residual = self._canvas("residual", 2, f_dec_batch if batched else f_dec,
+                                TensorWindow((2, T_, T_), (2, S_, S_)), dev, args=(latents,),
                                 args_windows=(TensorWindow((6, T_ // lc, T_ // lc), (6, S_ // lc, S_ // lc)),),
-                                cache_limit=lim)
+                                batch_size=self.decoder_batch_size if batched else None, cache_limit=lim)
         self._coarse, self._latents, self._residual = coarse, latents, residual
         wrap = _HostView if self._host_views else (lambda c: c)
         self.coarse, self.latents, self.residual = wrap(coarse), wrap(latents), wrap(residual)
@@ -675,7 +698,7 @@ class TerrainPipeline(WorldPipeline):
                  t_inter: float | None = None, residual_mean: float | None = None, residual_std: float | None = None,
                  native_resolution: float = 90.0, cache_limit: int | None = None, coarse_pooling: int = 1,
                  elev_coarse_pool_mode: str = "avg", p5_coarse_pool_mode: str = "avg", synthetic_map_stats=None,
-                 frequency_mult: list | None = None, coarse_batch_size: int = 1):
+                 frequency_mult: list | None = None, coarse_batch_size: int = 1, decoder_batch_size: int = 1):
         super().__init__(seed=seed, latents_batch_size=latents_batch_size, native_resolution=native_resolution,
                          latent_compression=latent_compression, cond_snr=[float(v) for v in cond_snr],
                          coarse_pooling=coarse_pooling, elev_coarse_pool_mode=elev_coarse_pool_mode,
@@ -687,7 +710,7 @@ class TerrainPipeline(WorldPipeline):
                          histogram_raw=[float(v) for v in torch.as_tensor(histogram_raw).flatten()],
                          cond_input_mean=[float(v) for v in torch.as_tensor(latents_means).flatten()],
                          cond_input_std=[float(v) for v in torch.as_tensor(latents_stds).flatten()], t_inter=t_inter,
-                         coarse_batch_size=coarse_batch_size)
+                         coarse_batch_size=coarse_batch_size, decoder_batch_size=decoder_batch_size)
         self.coarse_model, self.base_model, self.decoder_model = coarse_model, base_model, decoder_model
         self._host_views = False
         self._build_hierarchy()

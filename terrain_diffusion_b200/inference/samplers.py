@@ -74,14 +74,18 @@ def get_diffusion_solve(model, scheduler, n, h, w, num_steps, step_range=None, g
 
 
 def get_consistency_solve(model, n, h, w, t: float, sigma_data: float = 0.5, from_unit_noise: bool = False,
-                          out_scale: float = 1.0) -> DiffusionSolve:
-    """Cached one-step TrigFlow consistency program (solve.consistency_rows) for `n` tiles of h x w."""
+                          out_scale: float = 1.0, batch_invariant: bool = False) -> DiffusionSolve:
+    """Cached one-step TrigFlow consistency program (solve.consistency_rows) for `n` tiles of h x w.
+    batch_invariant: see DiffusionSolve."""
     from .solve import consistency_rows
     key = ("cm", n, h, w, float(t), float(sigma_data), bool(from_unit_noise), float(out_scale), id(model.folded()))
+    if batch_invariant:
+        key += ("batch_invariant",)
     cache = _solve_cache(model)
     if key not in cache:
         cache[key] = DiffusionSolve(model, None, n, h, w, 1,
-                                    coef_rows=consistency_rows(t, sigma_data, from_unit_noise, out_scale))
+                                    coef_rows=consistency_rows(t, sigma_data, from_unit_noise, out_scale),
+                                    batch_invariant=batch_invariant)
     return cache[key]
 
 

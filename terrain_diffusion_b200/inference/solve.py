@@ -61,7 +61,8 @@ class DiffusionSolve:
         decoder sampler, folded into the coefficient rows (fold_score_scaling).
         batch_invariant: each of the n tiles comes out bit-identical to a one-tile solve of it: the launches use their
         one-image item shapes (UNetEmitter), and the host embedding is computed for one tile and shared, so every
-        conditional input of run() must then be a single row."""
+        conditional input of run() must then be a single row.  A model that embeds its noise labels on the device
+        (the decoder) needs nothing more: the embed launch computes every row on its own."""
         fw = model.folded()
         dev = fw.device
         self.guided = guide is not None and float(guidance_scale) != 1.0

@@ -10,7 +10,8 @@ around the U-Net, `.item()`, D2H -- is organised here around ONE fused program p
                        the two scalars and the noise tile goes straight into the sample buffer; a later phase needs one
                        mixing launch (tdx_trig_mix).  The packed window output cat([x w, w]) is one launch
                        (tdx_pack_weighted); normalise-on-read + nearest upsampling of the latent window one launch
-                       (tdx_window_to_cond).
+                       (tdx_window_to_cond).  `decoder_stage_tiles` solves a batch of decoder windows with a
+                       batch-invariant program, so every window is bit-identical to its `decoder_stage_tile`.
   coarse stage         `get_diffusion_solve`: the 20-step DPM-Solver++ solve as one graph, the embeddings of all steps
                        from one batched call.  De-normalisation, the channel-1 difference, `coarse_pooling` and the
                        packed output are one launch (tdx_coarse_epilogue).  `coarse_stage_tiles` solves a batch of
@@ -89,6 +90,62 @@ def decoder_stage_tile(model, seed: int, ctx, latents: torch.Tensor, weight_wind
         x = z if k == 0 else trig_mix(sample, z, math.cos(t), math.sin(t) * sigma_data)
         sample = solve.run(x, cond)
     return pack_weighted(sample, _f32(weight_window, dev))[0]
+
+
+DECODER_BATCH_SIZES = (1, 2, 4)          # not 8 or 16: ~2 GB of activations per 512^2 window (DESIGN.md section 5)
+
+
+@torch.no_grad()
+def decoder_stage_tiles(model, seed: int, ctxs, latents_windows, weight_window: torch.Tensor, t_list,
+                        tile_size: int = 512, tile_stride: int = 384, sigma_data: float = 0.5,
+                        latent_compression: int = 8) -> list:
+    """decoder_stage_tile for a batch of windows: ctxs [(0, i, j), ...] with their packed [6, T/lc, T/lc] latent
+    windows (a list of CUDA or CPU tensors, or one [n, 6, T/lc, T/lc] tensor).  Returns the packed [2, T, T] windows
+    (views of one device tensor), each bit-identical to decoder_stage_tile of its window whatever the rest of the batch
+    is: every launch but the consistency program is elementwise, in that function's fp32 order, and the program is
+    batch-invariant.  The batch is padded to the next of DECODER_BATCH_SIZES by repeating window 0, so that few
+    programs exist per model.  At most DECODER_BATCH_SIZES[-1] windows per call."""
+    if len(ctxs) != len(latents_windows):                        # argument errors before any device work
+        raise ValueError(f"decoder_stage_tiles: {len(ctxs)} windows but {len(latents_windows)} latent windows")
+    top = DECODER_BATCH_SIZES[-1]
+    if len(ctxs) > top:
+        raise ValueError(f"decoder_stage_tiles: {len(ctxs)} windows, at most {top} per call")
+    T, lc = tile_size, latent_compression
+    want = (6, T // lc, T // lc)
+    if isinstance(latents_windows, torch.Tensor):
+        shapes = [tuple(latents_windows.shape[1:])] if latents_windows.dim() == 4 else [tuple(latents_windows.shape)]
+    else:
+        shapes = [tuple(torch.as_tensor(w).shape) for w in latents_windows]
+    bad = [s for s in shapes if s != want]
+    if bad:
+        raise ValueError(f"decoder_stage_tiles: latent windows must be {list(want)}, got {list(bad[0])}")
+    if not ctxs:
+        return []
+    dev = model.device
+    n = len(ctxs)
+    if isinstance(latents_windows, torch.Tensor):
+        lat = _f32(latents_windows, dev)
+    elif all(torch.as_tensor(w).device.type == "cpu" for w in latents_windows):     # host windows: ONE copy
+        lat = _f32(torch.stack([torch.as_tensor(w) for w in latents_windows]), dev)
+    else:
+        lat = torch.stack([_f32(torch.as_tensor(w), dev) for w in latents_windows])
+    origins = [(c[1] * tile_stride, c[2] * tile_stride) for c in ctxs]
+    m = padded_batch_size(n, top)
+    if m > n:      # padding repeats window 0 at the inputs: its condition and its noise
+        lat = torch.cat([lat, lat[:1].expand(m - n, -1, -1, -1)], dim=0)
+        origins += [origins[0]] * (m - n)
+    cond = window_to_cond(lat, 4, lc)
+    sample = None
+    for k, t in enumerate(t_list):
+        t = float(t)
+        z = gaussian_noise_patches(seed + 5819 + k, origins, T, T, 1, T, T, device=dev)
+        last = k == len(t_list) - 1
+        # one window: the program of decoder_stage_tile itself (a batch-invariant plan at one image is that plan)
+        solve = get_consistency_solve(model, m, T, T, t, sigma_data, from_unit_noise=(k == 0),
+                                      out_scale=1.0 / sigma_data if last else 1.0, batch_invariant=m > 1)
+        x = z if k == 0 else trig_mix(sample, z, math.cos(t), math.sin(t) * sigma_data)
+        sample = solve.run(x, cond)
+    return list(pack_weighted(sample[:n], _f32(weight_window, dev)))
 
 
 # ------------------------------------------------------------------------------------------------ latent stage
