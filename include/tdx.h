@@ -244,6 +244,19 @@ int tdx_coarse_epilogue(float* out, const float* x, const float* means, const fl
 int tdx_coarse_condition(float* cond, float* sample, const float* map, const float* cond_noise,
                          const float* sample_noise, const float* means, const float* stds, const float* cos_t,
                          const float* sin_t, float sigma0, int32_t n_img, int64_t plane, void* stream);
+/* The base model's embedding rows for n_rows latent tiles (world_pipeline.py:1018-1050 + edm_unet.py:145-159), one
+ * CTA per row and in a fixed fp32 order that does not depend on n_rows.  Row r reads the packed coarse window
+ * coarse[r] [7][4][4] (6 channels x w, then w) and computes the conditioning vector v [52 + n_tail]:
+ * x = nan_to_num((cat(coarse[:6] / coarse[6], 1) - cond_means) / cond_stds, nan=cond_means[0]) (+-inf -> +-FLT_MAX);
+ * v = cat(x[0], x[1], mean(x[2:6, 1:3, 1:3]), x[6], tail) * concat_scale, tail = histogram then noise level.
+ * Then emb[r] [emb_channels] = mp_silu((w_noise * pos_fourier(label) @ noise_weight + w_cond * mp_silu(v @ cond_weight))
+ * / w_norm), noise_weight [noise_dims][emb_channels] and cond_weight [52 + n_tail][emb_channels] transposed as
+ * FoldedWeights holds them.  cond_vec [n_rows][52 + n_tail] receives v when not NULL.  cond_means / cond_stds: 7 floats;
+ * noise_freqs: noise_dims / 2 floats; every pointer is a device pointer. */
+int tdx_latent_embed(float* emb, float* cond_vec, const float* coarse, const float* cond_means, const float* cond_stds,
+                     const float* tail, int32_t n_tail, const float* concat_scale, const float* noise_freqs,
+                     const float* noise_weight, const float* cond_weight, int32_t noise_dims, int32_t emb_channels,
+                     float label, float w_noise, float w_cond, float w_norm, int32_t n_rows, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Elevation read-out (WorldPipeline._compute_elev, inference/world_pipeline.py:1277-1313): the reference normalises

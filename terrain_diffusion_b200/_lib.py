@@ -233,6 +233,10 @@ def _declare(l: C.CDLL) -> None:
     l.tdx_coarse_condition.restype = C.c_int
     l.tdx_coarse_condition.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int32, C.c_int64, C.c_void_p]
+    l.tdx_latent_embed.restype = C.c_int
+    l.tdx_latent_embed.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_float,
+                                   C.c_float, C.c_float, C.c_float, C.c_int32, C.c_void_p]
     l.tdx_noise_patches_workspace_bytes.restype = C.c_int64
     l.tdx_noise_patches_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     l.tdx_standard_normal.restype = C.c_int

@@ -8,7 +8,7 @@ from .sharded import ShardedCanvas  # noqa: F401
 from .solve import DiffusionSolve, fold_score_scaling  # noqa: F401
 from .tiling import linear_weight_window, padded_batch_size, shard_rows, tile_starts, window_range  # noqa: F401
 from .stages import (coarse_epilogue, coarse_geometry, coarse_stage_tile, decoder_stage_tile,  # noqa: F401
-                     decoder_stage_tiles, latent_stage_tiles, process_latent_conditioning)
+                     decoder_stage_tiles, latent_embedding, latent_stage_tiles, process_latent_conditioning)
 from .lazy_canvas import LazyCanvas, TensorWindow  # noqa: F401
 from .pipeline import TerrainPipeline, WorldPipeline  # noqa: F401
 from .relief import get_relief_map  # noqa: F401

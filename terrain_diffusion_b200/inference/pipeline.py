@@ -35,6 +35,13 @@ config.json.  Any other value raises ValueError in the constructor.
 `decoder_batch_size = b` (one of stages.DECODER_BATCH_SIZES, keyword-only; default 1) does the same for the decoder
 stage: up to b missing residual windows per call (`stages.decoder_stage_tiles`), each bit-identical to its one-window
 solve.  Its consistency program holds b windows of activations (DESIGN.md section 5 gives the measured memory).
+
+`latents_batch_invariant = True` (keyword-only; default False) solves every latent tile bit-identically to its one-tile
+solve (`stages.latent_stage_tiles(batch_invariant=True)`): its embedding row is computed on the device from its own
+coarse window and its program is planned at a fixed anchor, the largest `latents_batch_size`.  With it, what a world
+reads is a function of seed, configuration and coordinates only, whatever the request order, the cache evictions,
+`coarse_batch_size` and `decoder_batch_size`.  The bits depend on the largest `latents_batch_size`, and differ from
+those of the default path in the last places.  It is not written to config.json.
 """
 from __future__ import annotations
 
@@ -49,8 +56,9 @@ import torch
 from ..scheduler import EDMDPMSolverMultistepScheduler
 from .lazy_canvas import LazyCanvas, TensorWindow
 from .stages import (COARSE_BATCH_SIZES, DECODER_BATCH_SIZES, coarse_geometry, coarse_stage_tile, coarse_stage_tiles,
-                     decoder_stage_tile, decoder_stage_tiles, latent_stage_tiles)
-from .tiling import linear_weight_window
+                     decoder_stage_tile, decoder_stage_tiles, latent_embed_spec, latent_plan_images,
+                     latent_stage_tiles)
+from .tiling import linear_weight_window, padded_batch_size
 
 # seed offsets of the latent stage's noise fields: _build_latent_stage (world_pipeline.py:1133-1203) passes 5819 to the
 # init phase and 5820 + i to the i-th T_INTER phase (pinned against the reference source by tests/golden/stages_golden.npz)
@@ -92,8 +100,9 @@ class WorldPipeline:
     BASE_MODEL_FOLDER = "base_model"
     DECODER_MODEL_FOLDER = "decoder_model"
     config_name = "config.json"
-    ignore_for_config = ["seed", "latents_batch_size", "coarse_batch_size", "decoder_batch_size", "log_mode",
-                         "cache_limit", "caching_strategy", "torch_compile", "dtype"]
+    ignore_for_config = ["seed", "latents_batch_size", "coarse_batch_size", "decoder_batch_size",
+                         "latents_batch_invariant", "log_mode", "cache_limit", "caching_strategy", "torch_compile",
+                         "dtype"]
 
     def __init__(self, seed: int | None = None, latents_batch_size=(1, 2, 4, 8, 16), native_resolution: float = 90.0, *,
                  T: int = 2, log_mode: str = "info", torch_compile: bool = False, dtype: str | None = None,
@@ -104,7 +113,7 @@ class WorldPipeline:
                  cache_limit: int | None = 100 * 1024 * 1024, onestep_latent: bool = False,
                  decoder_tile_size: int = 512, decoder_tile_stride: int = 384, conditioning_fn=None,
                  synthetic_map_stats=None, coarse_batch_size: int = 1, decoder_batch_size: int = 1,
-                 **deprecated_kwargs):
+                 latents_batch_invariant: bool = False, **deprecated_kwargs):
         from .noise import next_seed
         if T not in (1, 2):
             raise ValueError(f"T must be 1 or 2, got {T}")
@@ -114,6 +123,9 @@ class WorldPipeline:
         coarse_pooling = operator.index(coarse_pooling)
         self.coarse_batch_size = _batch_size("coarse_batch_size", coarse_batch_size, COARSE_BATCH_SIZES)
         self.decoder_batch_size = _batch_size("decoder_batch_size", decoder_batch_size, DECODER_BATCH_SIZES)
+        if not isinstance(latents_batch_invariant, bool):
+            raise ValueError(f"latents_batch_invariant must be True or False; got {latents_batch_invariant!r}")
+        self.latents_batch_invariant = latents_batch_invariant
         self.T = T
         self.seed = (int(seed) & 0xFFFFFFFFFFFFFFFF) if seed is not None else next_seed(None)
         sizes = [latents_batch_size] if isinstance(latents_batch_size, int) else sorted(latents_batch_size)
@@ -242,10 +254,20 @@ class WorldPipeline:
         sd = 0.5
         if self.base_model is not None:
             phases = [(self.t_init, True)] + ([] if self.onestep_latent else [(self.t_inter, False)])
-            for m in self._batch_sizes:
-                for t, first in phases:
-                    get_consistency_solve(self.base_model, int(m), 64, 64, float(t), sd, from_unit_noise=first,
-                                          out_scale=1.0 / sd).prog.instantiate()
+            if self.latents_batch_invariant:
+                # the anchored programs at every size latent_stage_tiles pads a batch to
+                top = self.latents_batch_size
+                latent_embed_spec(self.base_model)
+                for m in sorted({padded_batch_size(k, top) for k in range(1, top + 1)}):
+                    for t, first in phases:
+                        get_consistency_solve(self.base_model, m, 64, 64, float(t), sd, from_unit_noise=first,
+                                              out_scale=1.0 / sd, batch_invariant=True,
+                                              plan_images=latent_plan_images(top)).prog.instantiate()
+            else:
+                for m in self._batch_sizes:
+                    for t, first in phases:
+                        get_consistency_solve(self.base_model, int(m), 64, 64, float(t), sd, from_unit_noise=first,
+                                              out_scale=1.0 / sd).prog.instantiate()
         if self.decoder_model is not None:
             T_ = self.decoder_tile_size
             get_consistency_solve(self.decoder_model, 1, T_, T_, float(self.t_init), sd, from_unit_noise=True,
@@ -385,14 +407,17 @@ class WorldPipeline:
                               batch_size=self.coarse_batch_size if batched else None, cache_limit=lim)
 
         # ---- latents: 64^2 tiles, stride 32; T=2: two consistency phases with a blend in between, T=1: both phases per
-        # tile; batches padded to the legal sizes so that only a handful of plans exist
+        # tile; batches padded to the legal sizes so that only a handful of plans exist.  latents_batch_invariant: each
+        # tile is bit-identical to its one-tile solve (stages.latent_stage_tiles), so the canvas does not depend on
+        # which tiles were computed together
         out_w = TensorWindow((6, 64, 64), (6, 32, 32))
         coarse_w = TensorWindow((7, 4, 4), (7, 1, 1), (0, -1, -1))
         pad = self.latents_batch_size
 
         def phase(ctxs, prev, conds, t, off):
             return latent_stage_tiles(self.base_model, self.seed, ctxs, prev, conds, t, ww64, hist, self.cond_input_mean,
-                                      self.cond_input_std, seed_offset=off, pad_batch_to=pad)
+                                      self.cond_input_std, seed_offset=off, pad_batch_to=pad,
+                                      batch_invariant=self.latents_batch_invariant)
 
         if self.T == 1:
             def f_t1(ctxs, conds):
@@ -698,7 +723,8 @@ class TerrainPipeline(WorldPipeline):
                  t_inter: float | None = None, residual_mean: float | None = None, residual_std: float | None = None,
                  native_resolution: float = 90.0, cache_limit: int | None = None, coarse_pooling: int = 1,
                  elev_coarse_pool_mode: str = "avg", p5_coarse_pool_mode: str = "avg", synthetic_map_stats=None,
-                 frequency_mult: list | None = None, coarse_batch_size: int = 1, decoder_batch_size: int = 1):
+                 frequency_mult: list | None = None, coarse_batch_size: int = 1, decoder_batch_size: int = 1,
+                 latents_batch_invariant: bool = False):
         super().__init__(seed=seed, latents_batch_size=latents_batch_size, native_resolution=native_resolution,
                          latent_compression=latent_compression, cond_snr=[float(v) for v in cond_snr],
                          coarse_pooling=coarse_pooling, elev_coarse_pool_mode=elev_coarse_pool_mode,
@@ -710,7 +736,8 @@ class TerrainPipeline(WorldPipeline):
                          histogram_raw=[float(v) for v in torch.as_tensor(histogram_raw).flatten()],
                          cond_input_mean=[float(v) for v in torch.as_tensor(latents_means).flatten()],
                          cond_input_std=[float(v) for v in torch.as_tensor(latents_stds).flatten()], t_inter=t_inter,
-                         coarse_batch_size=coarse_batch_size, decoder_batch_size=decoder_batch_size)
+                         coarse_batch_size=coarse_batch_size, decoder_batch_size=decoder_batch_size,
+                         latents_batch_invariant=latents_batch_invariant)
         self.coarse_model, self.base_model, self.decoder_model = coarse_model, base_model, decoder_model
         self._host_views = False
         self._build_hierarchy()

@@ -74,18 +74,21 @@ def get_diffusion_solve(model, scheduler, n, h, w, num_steps, step_range=None, g
 
 
 def get_consistency_solve(model, n, h, w, t: float, sigma_data: float = 0.5, from_unit_noise: bool = False,
-                          out_scale: float = 1.0, batch_invariant: bool = False) -> DiffusionSolve:
+                          out_scale: float = 1.0, batch_invariant: bool = False,
+                          plan_images: int = 1) -> DiffusionSolve:
     """Cached one-step TrigFlow consistency program (solve.consistency_rows) for `n` tiles of h x w.
-    batch_invariant: see DiffusionSolve."""
+    batch_invariant, plan_images: see DiffusionSolve."""
     from .solve import consistency_rows
     key = ("cm", n, h, w, float(t), float(sigma_data), bool(from_unit_noise), float(out_scale), id(model.folded()))
+    if plan_images != 1:
+        key += ("plan_images", int(plan_images))
     if batch_invariant:
         key += ("batch_invariant",)
     cache = _solve_cache(model)
     if key not in cache:
         cache[key] = DiffusionSolve(model, None, n, h, w, 1,
                                     coef_rows=consistency_rows(t, sigma_data, from_unit_noise, out_scale),
-                                    batch_invariant=batch_invariant)
+                                    batch_invariant=batch_invariant, plan_images=plan_images)
     return cache[key]
 
 

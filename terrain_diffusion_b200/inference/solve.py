@@ -50,7 +50,8 @@ class DiffusionSolve:
     exactly the unguided program (the reference skips the guide forward then too)."""
 
     def __init__(self, model, scheduler, n: int, h: int, w: int, num_steps: int, step_range=None, coef_rows=None,
-                 guide=None, guidance_scale: float = 1.0, score_scaling: float = 1.0, batch_invariant: bool = False):
+                 guide=None, guidance_scale: float = 1.0, score_scaling: float = 1.0, batch_invariant: bool = False,
+                 plan_images: int = 1):
         """coef_rows: explicit per-step tables [dict(c_in, t, c_skip, c_out, r, k)] instead of a scheduler's (the
         TrigFlow consistency step is the same fused program with other numbers: consistency_rows()).
         step_range = (i0, i1): only steps i0 .. i1-1 of the `num_steps` schedule (one PHASE of a multi-phase
@@ -62,7 +63,12 @@ class DiffusionSolve:
         batch_invariant: each of the n tiles comes out bit-identical to a one-tile solve of it: the launches use their
         one-image item shapes (UNetEmitter), and the host embedding is computed for one tile and shared, so every
         conditional input of run() must then be a single row.  A model that embeds its noise labels on the device
-        (the decoder) needs nothing more: the embed launch computes every row on its own."""
+        (the decoder) needs nothing more: the embed launch computes every row on its own.
+        plan_images: the image count a batch-invariant solve plans its launches at (UNetEmitter); every solve with the
+        same anchor gives a tile the same bits.  A caller that computes each row's embedding on the device itself
+        (the latent stage, stages.latent_embedding) writes `emb_all` and calls run(..., embedding_ready=True)."""
+        if plan_images != 1 and not batch_invariant:
+            raise ValueError("plan_images applies to batch-invariant solves only")
         fw = model.folded()
         dev = fw.device
         self.guided = guide is not None and float(guidance_scale) != 1.0
@@ -109,12 +115,12 @@ class DiffusionSolve:
         self.x0_prev = torch.zeros_like(self.sample)
         self.prog = UNetProgram(fw.device)
         # the noise labels of all steps are known up front: ONE embed launch produces every step's modulation vectors
-        em = UNetEmitter(fw, n, h, w, cvec_sets=num_steps, batch_invariant=batch_invariant)
+        em = UNetEmitter(fw, n, h, w, cvec_sets=num_steps, batch_invariant=batch_invariant, plan_images=plan_images)
         self.host_emb = len(model.conditional_layers) > 0 or not fw.pos_emb
         if self.guided:
             check_plannable(gfw, "guide model")
             gem = UNetEmitter(gfw, n, h, w, cvec_sets=num_steps,          # its own arena and modulation vectors
-                              batch_invariant=batch_invariant)
+                              batch_invariant=batch_invariant, plan_images=plan_images)
             self.guide_out = torch.zeros_like(self.sample)
         if self.host_emb:
             # conditional models (coarse: five float conditions): the 256-wide embeddings of all steps are computed
@@ -145,10 +151,18 @@ class DiffusionSolve:
 
     @torch.no_grad()
     def run(self, noise: torch.Tensor, cond: torch.Tensor | None, use_graph: bool = True,
-            conditional_inputs=None) -> torch.Tensor:
+            conditional_inputs=None, embedding_ready: bool = False) -> torch.Tensor:
         """noise: [n, Cs, h, w] initial sample (already scaled by sigma_0); returns the denoised sample (a view of the
-        solver's state buffer -- copy it before the next run)."""
-        if self.host_emb:
+        solver's state buffer -- copy it before the next run).  embedding_ready: the caller has written every row of
+        `emb_all` itself (device-computed embeddings, one per tile and step), so no host embedding is computed and
+        conditional_inputs must be None."""
+        if embedding_ready:
+            if not self.host_emb or self.guided:
+                raise ValueError("embedding_ready needs an unguided solve of a model that takes its embedding rows "
+                                 "from emb_all")
+            if conditional_inputs is not None:
+                raise ValueError("embedding_ready: the embedding rows already hold the conditional inputs")
+        elif self.host_emb:
             # conditional models: ONE batched evaluation of compute_embeddings for the labels of all steps
             labels = self.labels[:, :1].reshape(-1) if self.batch_invariant else self.labels.reshape(-1)
             if self.batch_invariant and any(c.shape[0] != 1 for c in (conditional_inputs or [])):

@@ -17,6 +17,9 @@ around the U-Net, `.item()`, D2H -- is organised here around ONE fused program p
                        packed output are one launch (tdx_coarse_epilogue).  `coarse_stage_tiles` solves a batch of
                        windows: its inputs are one launch (tdx_coarse_condition) and its solve is batch-invariant, so
                        every window is bit-identical to its `coarse_stage_tile`.
+  latent stage         `latent_stage_tiles`: one consistency phase of a padded batch of 64^2 tiles.  With
+                       batch_invariant=True every tile's embedding row is one CTA of tdx_latent_embed and the program is
+                       planned at a fixed anchor, so every tile is bit-identical to a one-tile call of itself.
 
 Noise comes from the bit-compatible GPU generator (same seeds as the reference), nothing synchronises with the host and
 nothing leaves the GPU.  Taken as arguments: the synthetic conditioning map of the coarse stage (built on the device by
@@ -210,13 +213,112 @@ def process_latent_conditioning(cond_img, histogram_raw, cond_means, cond_stds, 
     return torch.cat(parts, dim=1) * _concat_scales([p.shape[1] for p in parts], dev)
 
 
+LATENT_BATCH_SIZES = (1, 2, 4, 8, 16)
+LATENT_EMBED_MAX_CHANNELS = 1024         # tdx_latent_embed: one CTA per row, the row's embedding in registers
+
+
+def latent_embed_spec(model) -> dict:
+    """What tdx_latent_embed needs to know of the base model, read from its config: a positional noise embedding (its
+    dims a multiple of 4, at most 512), exactly one `tensor` conditional input of 52 + n_tail values and at most 1024
+    embedding channels, and the mp_sum weights of the two embeddings in fp32 as _host_embedding uses them.  Any other
+    embedding configuration raises ValueError."""
+    cfg = dict(model.config)
+    conds = [list(c) for c in (cfg.get("conditional_inputs") or [])]
+    mults = cfg.get("model_channel_mults") or [1, 2, 3, 4]
+    mc = cfg.get("model_channels", 128)
+    noise_dims = mc if cfg.get("noise_emb_dims") is None else cfg["noise_emb_dims"]
+    emb = cfg.get("emb_channels") or mc * max(mults)
+    if (cfg.get("fourier_scale") != "pos" or not 4 <= noise_dims <= 512 or noise_dims % 4 or len(conds) != 1
+            or conds[0][0] != "tensor" or not 53 <= int(conds[0][1]) <= 128 or emb > LATENT_EMBED_MAX_CHANNELS):
+        raise ValueError("the batch-invariant latent stage embeds on the device and supports a positional noise "
+                         "embedding (a multiple of 4 dims, at most 512), one 'tensor' conditional input of 53..128 "
+                         f"values and at most {LATENT_EMBED_MAX_CHANNELS} embedding channels; this model has "
+                         f"fourier_scale={cfg.get('fourier_scale')!r}, noise_emb_dims={noise_dims}, "
+                         f"conditional_inputs={conds}, emb_channels={emb}")
+    w32 = torch.tensor([1.0, float(conds[0][2])], dtype=torch.float32)   # _host_embedding's mp_sum weights and norm
+    return dict(noise_dims=int(noise_dims), emb_channels=int(emb), cond_dims=int(conds[0][1]), w_noise=float(w32[0]),
+                w_cond=float(w32[1]), w_norm=float(torch.linalg.vector_norm(w32)))
+
+
+def latent_plan_images(top: int) -> int:
+    """The image count the batch-invariant latent programs plan their launches at (the anchor): the largest padded
+    batch, so that a full batch runs its free plan (DESIGN.md section 5 gives the measurement behind the choice)."""
+    return int(top)
+
+
+def latent_embedding(model, coarse: torch.Tensor, histogram_raw, cond_means, cond_stds, t: float, out: torch.Tensor,
+                     cond_vec: torch.Tensor | None = None) -> torch.Tensor:
+    """The base model's embedding rows of n latent tiles in one launch (tdx_latent_embed): coarse [n, 7, 4, 4] packed
+    coarse windows (contiguous fp32 on the model's device) -> out [n, E], row r a function of coarse[r] alone.  What
+    latent_stage_tiles + process_latent_conditioning + EDMUnet2D._host_embedding compute, at noise level 0 and label t,
+    in one fixed fp32 order per row.  histogram_raw: [H] or [1, H], shared by every row.  cond_vec [n, 52 + H + 1]
+    receives the conditioning vectors when given."""
+    spec = latent_embed_spec(model)
+    fw = model.folded()
+    dev = coarse.device
+    n = coarse.shape[0]
+    hist = torch.as_tensor(histogram_raw, dtype=torch.float32).cpu().reshape(-1)
+    level = ((torch.tensor(0.0, dtype=torch.float32) - 0.5) * math.sqrt(12)).reshape(1)   # process_latent_conditioning's
+    tail = _const_on(dev, torch.cat([hist, level]))
+    dims = [16, 16, 4, 16, hist.numel(), 1]
+    if sum(dims) != spec["cond_dims"]:
+        raise ValueError(f"latent_embedding: {hist.numel()} histogram values make a {sum(dims)}-value conditioning "
+                         f"vector; the model takes {spec['cond_dims']}")
+    E = spec["emb_channels"]
+    for name, ten, shape in (("coarse", coarse, (n, 7, 4, 4)), ("out", out, (n, E)),
+                             ("cond_vec", cond_vec, (n, sum(dims)))):
+        if ten is not None and (tuple(ten.shape) != shape or ten.dtype != torch.float32 or not ten.is_contiguous()
+                                or ten.device != fw.device):
+            raise ValueError(f"latent_embedding: {name} must be a contiguous fp32 {list(shape)} tensor on "
+                             f"{fw.device}, got {ten.dtype} {tuple(ten.shape)} on {ten.device}")
+    g = fw.g
+    L.call(L.lib().tdx_latent_embed, dev, out.data_ptr(), None if cond_vec is None else cond_vec.data_ptr(),
+           coarse.data_ptr(), _const_on(dev, cond_means).data_ptr(), _const_on(dev, cond_stds).data_ptr(),
+           tail.data_ptr(), tail.numel(), _concat_scales(dims, dev).data_ptr(), g["noise_freqs"].data_ptr(),
+           g["noise_linear"].data_ptr(), g["cond0"].data_ptr(), spec["noise_dims"], E, float(t), spec["w_noise"],
+           spec["w_cond"], spec["w_norm"], n)
+    return out
+
+
+def _check_latent_arguments(model, ctxs, samples, cond_imgs, histogram_raw, top: int) -> None:
+    """The batch-invariant latent stage's argument errors, raised before any device work."""
+    n = len(ctxs)
+    if len(cond_imgs) != n:
+        raise ValueError(f"latent_stage_tiles: {n} tiles but {len(cond_imgs)} coarse windows")
+    if samples is not None and len(samples) != n:
+        raise ValueError(f"latent_stage_tiles: {n} tiles but {len(samples)} samples")
+    if n > top:
+        raise ValueError(f"latent_stage_tiles: {n} tiles, at most {top} per batch-invariant call")
+    bad = [tuple(torch.as_tensor(c).shape) for c in cond_imgs if tuple(torch.as_tensor(c).shape) != (7, 4, 4)]
+    if bad:
+        raise ValueError(f"latent_stage_tiles: coarse windows must be [7, 4, 4], got {list(bad[0])}")
+    shapes = [tuple(torch.as_tensor(s).shape) for s in (samples or []) if s is not None]
+    bad = [sh for sh in shapes if sh != (6, LATENT_TILE, LATENT_TILE)]
+    if bad:
+        raise ValueError(f"latent_stage_tiles: samples must be [6, {LATENT_TILE}, {LATENT_TILE}], got {list(bad[0])}")
+    if 0 < len(shapes) < n:
+        raise ValueError("latent_stage_tiles: samples must be all None (first phase) or all windows")
+    hist = torch.as_tensor(histogram_raw)
+    if hist.dim() > 2 or (hist.dim() == 2 and hist.shape[0] != 1):
+        raise ValueError(f"latent_stage_tiles: the batch-invariant stage takes one shared histogram ([H] or [1, H]), "
+                         f"got {list(hist.shape)}")
+    latent_embed_spec(model)
+
+
 @torch.no_grad()
 def latent_stage_tiles(model, seed: int, ctxs, samples, cond_imgs, t: float, weight_window: torch.Tensor,
                        histogram_raw, cond_means, cond_stds, seed_offset: int = 0, sigma_data: float = 0.5,
-                       pad_batch_to=None) -> list:
+                       pad_batch_to=None, batch_invariant: bool = False) -> list:
     """One consistency phase of the latent stage for a batch of window indices (world_pipeline.py:1052-1131).
     samples: None (first phase) or packed [6, 64, 64] windows of the previous phase's canvas; cond_imgs: packed
-    [7, 4, 4] coarse windows.  Returns the packed [6, 64, 64] tiles (views of one device tensor)."""
+    [7, 4, 4] coarse windows.  Returns the packed [6, 64, 64] tiles (views of one device tensor).
+    batch_invariant: every tile comes out bit-identical to a one-tile call of itself, whatever else is in the batch.
+    Its embedding rows are computed on the device per tile (latent_embedding) and the program is planned at the
+    anchor latent_plan_images(top), top = pad_batch_to or 16, at every padded batch size; so a tile's bits depend on
+    top (the pipeline's largest latents_batch_size) and at most top tiles are taken per call."""
+    if batch_invariant:
+        top = int(pad_batch_to or LATENT_BATCH_SIZES[-1])
+        _check_latent_arguments(model, ctxs, samples, cond_imgs, histogram_raw, top)
     if not ctxs:
         return []
     dev = model.device
@@ -227,8 +329,9 @@ def latent_stage_tiles(model, seed: int, ctxs, samples, cond_imgs, t: float, wei
         coarse = _f32(torch.stack(cond_imgs), dev)
     else:
         coarse = torch.stack([_f32(c, dev) for c in cond_imgs])                                  # [n, 7, 4, 4] packed
-    cimg = torch.cat([coarse[:, :-1] / coarse[:, -1:], torch.ones((n, 1, 4, 4), device=dev)], dim=1)
-    cvec = process_latent_conditioning(cimg, histogram_raw, cond_means, cond_stds, torch.tensor(0.0))
+    if not batch_invariant:
+        cimg = torch.cat([coarse[:, :-1] / coarse[:, -1:], torch.ones((n, 1, 4, 4), device=dev)], dim=1)
+        cvec = process_latent_conditioning(cimg, histogram_raw, cond_means, cond_stds, torch.tensor(0.0))
     z = gaussian_noise_patches(seed + seed_offset, [(c[1] * LATENT_STRIDE, c[2] * LATENT_STRIDE) for c in ctxs], T, T, 5,
                                T, T, device=dev)
     first = samples is None or all(s is None for s in samples)
@@ -237,6 +340,16 @@ def latent_stage_tiles(model, seed: int, ctxs, samples, cond_imgs, t: float, wei
     else:
         prev = torch.stack([_f32(torch.as_tensor(s), dev) for s in samples])                     # [n, 6, T, T] packed
         x = trig_mix(window_to_cond(prev, 5, 1), z, math.cos(t) * sigma_data, math.sin(t) * sigma_data)
+    if batch_invariant:
+        m = padded_batch_size(n, top)
+        if m > n:  # padding repeats tile 0 at the inputs; the anchored program keeps the real tiles' bits
+            x = torch.cat([x, x[:1].expand(m - n, -1, -1, -1)], dim=0)
+            coarse = torch.cat([coarse, coarse[:1].expand(m - n, -1, -1, -1)], dim=0)
+        solve = get_consistency_solve(model, m, T, T, t, sigma_data, from_unit_noise=first, out_scale=1.0 / sigma_data,
+                                      batch_invariant=True, plan_images=latent_plan_images(top))
+        latent_embedding(model, coarse.contiguous(), histogram_raw, cond_means, cond_stds, t, solve.emb_all)
+        sample = solve.run(x, None, embedding_ready=True)
+        return list(pack_weighted(sample[:n], _f32(weight_window, dev)))
     m = padded_batch_size(n, pad_batch_to) if pad_batch_to else n
     if m > n:   # the reference pads to {1,2,4,8,16} under torch.compile (:393-398, 1107-1118): one plan per size
         x = torch.cat([x, x[:1].expand(m - n, -1, -1, -1)], dim=0)

@@ -318,13 +318,18 @@ class UNetProgram:
 class UNetEmitter:
     """Allocates the activation arena for (n, h, w) and appends the launches of one U-Net evaluation to a program."""
 
-    def __init__(self, fw: FoldedWeights, n: int, h: int, w: int, cvec_sets: int = 1, batch_invariant: bool = False):
+    def __init__(self, fw: FoldedWeights, n: int, h: int, w: int, cvec_sets: int = 1, batch_invariant: bool = False,
+                 plan_images: int = 1):
         """cvec_sets: how many independent label sets (e.g. solver steps) share this arena; the modulation vectors of
         all of them are produced by ONE embed launch (emit_embed) and selected per evaluation with `cvec_set`.
-        batch_invariant: every implicit-GEMM launch uses the item shape (N, split-K) its one-image plan would, the
-        other images as extra M tiles, so each image's result is bit-identical to a one-image program's."""
+        batch_invariant: every implicit-GEMM launch uses the item shape (N, split-K) its plan at `plan_images` images
+        would (the anchor; one image by default), whatever n is, so each image's result is bit-identical to that of
+        any other program with the same anchor."""
         self.cvec_sets = cvec_sets
         self.batch_invariant = batch_invariant
+        self.plan_images = int(plan_images)
+        if self.plan_images < 1:
+            raise ValueError(f"plan_images must be at least 1, got {plan_images!r}")
         downs = sum(b.get("resample") == "down" for b in fw.enc)
         ups = sum(b.get("resample") == "up" for b in fw.dec)
         need = 8 * 2 ** downs
@@ -413,7 +418,8 @@ class UNetEmitter:
             d.a_channels[i] = ch
             d.a_taps[i] = taps
         d.n_seg = len(segs)
-        n_item = L.igemm_choose_n(cout, 1 if self.batch_invariant else self.n, h, w, [(ch, taps) for _, ch, taps in segs])
+        n_item = L.igemm_choose_n(cout, self.plan_images if self.batch_invariant else self.n, h, w,
+                                  [(ch, taps) for _, ch, taps in segs])
         d.n_per_item = n_item
         d.b_packed = self.fw.packed(wkey, n_item).data_ptr()
         d.c_out = cout
@@ -423,7 +429,7 @@ class UNetEmitter:
     def _add_igemm(self, prog, d):
         if self.batch_invariant:
             one = L.TdxIgemmDesc.from_buffer_copy(d)
-            one.n_img, one.ksplit = 1, 0
+            one.n_img, one.ksplit = self.plan_images, 0
             d.ksplit = L.igemm_launch_shape(one)[1]
         prog.add("igemm", d)
 
